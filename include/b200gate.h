@@ -71,8 +71,11 @@ typedef struct b200gate_params {
                                  * cp.async (measured: no gain); bit 4: two units per warp in the n_fft 1024 FFT kernels
                                  * (the dual forms) instead of one; bit 5: tile-based float-mask smoothing;
                                  * bit 6: the non-stationary follower stores its forward sweep instead of regenerating
-                                 * it; bit 7: tap-loop float-mask smoothing instead of the box-sum form.  (bit 0 selected
-                                 * a single-pass experiment that was removed; it is ignored)                          */
+                                 * it; bit 7: tap-loop float-mask smoothing instead of the box-sum form; bit 8: stationary
+                                 * gate, smooth the binary mask in a separate kernel that stores 16-bit numerators for the
+                                 * synthesis kernel to read, instead of inside the synthesis kernel (same integers, more
+                                 * workspace and HBM traffic).  (bit 0 selected a single-pass experiment that was removed;
+                                 * it is ignored)                                                                      */
     int64_t chunk_size;         /* <= 0: never chunk (torch surface / chunk_size=None)           */
     int64_t padding;
     double sr;

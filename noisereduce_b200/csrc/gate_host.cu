@@ -2,7 +2,8 @@
 //
 // The planner turns the reference's chunk loop (noisereduce/spectralgate/base.py:167-226) into a
 // table of independent (chunk, channel) units, sizes the device workspace, and launches
-// k1_analyze -> k_rowfloor -> k_smooth -> k2_synthesize per batch of units on the caller's stream.
+// k1_analyze -> k_rowfloor -> [k_smooth] -> k2_synthesize per batch of units on the caller's stream (the stationary
+// gate's default synthesis kernel smooths the mask itself; k_smooth runs on the fallback paths).
 #include "../../include/b200gate.h"
 #include "gate_kernels_2k.cuh"
 #include "gate_synth.cuh"
@@ -669,6 +670,23 @@ void launch_k1n(const Geom& g, const Tables& tb, const void* x, int kdt, float* 
                     k1n_smem_floats() * 4, st, a1); });
 }
 
+// Binary-mask smoothing in byte lanes (k_smooth_packed, k2c_synthesize kMaskBits*): time sums up to (nt+1)^2 <= 196 per
+// byte, biased first differences <= 31, at most 36 frequency taps; k_smooth_generic takes the rest.
+static bool packed_smoothing_fits(int nf, int nt) { return nt + 1 <= 14 && 2 * nf + 1 <= 36; }
+
+// k2c_synthesize kMaskBits*: a time-sum row keeps bin k at byte sm_pad + k with sm_pad a multiple of 16 (one 16-byte store
+// per lane), so the tap window of bin 4i+j starts at byte 4 (i + sm_ws) + lead + j: the taps carry `lead` zero bytes first.
+static void set_k2c_smoothing_taps(K2Args& a, int nf) {
+    a.sm_pad = (nf + 15) & ~15;
+    const int off = a.sm_pad - nf, lead = off & 3;
+    a.sm_ws = off >> 2;
+    const int words = (2 * nf + 1 + lead + 3) / 4;
+    a.sm_ntw = words <= 4 ? 4 : words <= 7 ? 7 : words <= 9 ? 9 : kSynMaxTapWords;
+    unsigned char tb8[4 * kSynMaxTapWords] = {0};
+    for (int d = -nf; d <= nf; ++d) tb8[lead + d + nf] = (unsigned char)(nf + 1 - abs(d));
+    memcpy(a.sm_taps, tb8, sizeof tb8);
+}
+
 // Float-mask smoothing (non-stationary gate, TorchGate moving-mean gate): the box form for 1 <= nf <= 12 (k_smooth_box,
 // compiled per nf), else the tap-loop streaming kernel, else (ring too large for shared memory) the tile kernel.
 #define B200_SMOOTH_BOX_CASE(NF_) case NF_: { auto kern_ = k_smooth_box<NF_>; \
@@ -902,6 +920,8 @@ int b200gate_create(const b200gate_params* p, b200gate_handle** out) {
                 cudaFuncSetAttribute(k2c_synthesize<8, kMaskU16, T>, cudaFuncAttributeMaxDynamicSharedMemorySize, k2c_smem_bytes<kMaskU16>());
                 cudaFuncSetAttribute(k2c_synthesize<8, kMaskU16Blend, T>, cudaFuncAttributeMaxDynamicSharedMemorySize, k2c_smem_bytes<kMaskU16Blend>());
                 cudaFuncSetAttribute(k2c_synthesize<8, kMaskF32, T>, cudaFuncAttributeMaxDynamicSharedMemorySize, k2c_smem_bytes<kMaskF32>());
+                cudaFuncSetAttribute(k2c_synthesize<8, kMaskBits, T>, cudaFuncAttributeMaxDynamicSharedMemorySize, k2c_smem_bytes<kMaskBits>());
+                cudaFuncSetAttribute(k2c_synthesize<8, kMaskBitsBlend, T>, cudaFuncAttributeMaxDynamicSharedMemorySize, k2c_smem_bytes<kMaskBitsBlend>());
             });
         cudaFuncSetAttribute(k1_analyze<8, float, true>, cudaFuncAttributeMaxDynamicSharedMemorySize, k1_smem_floats_staged() * 4);
         cudaFuncSetAttribute(k_smooth_f, cudaFuncAttributeMaxDynamicSharedMemorySize, 200 * 1024);
@@ -1329,9 +1349,6 @@ int b200gate_run(b200gate_handle* h, const void* in, void* out, int dtype, int64
 
     // ---- workspace / batching ---------------------------------------------------------------------
     const bool stat = p.stationary != 0;
-    const size_t per_unit_2pass = (stat ? (size_t)g.T * kFW * 4 + (size_t)kFPad * 4 + (size_t)kFW * 4 + (size_t)num_unit_stride(g.T) * 2 + 64
-                                        : 2 * (size_t)g.T * FP * 4 + 64) +
-                                  (stat && torch_sem ? (size_t)g.T * kFPad * 4 + 2 * (size_t)kFPad * 4 : 0) + 2048;
     // spectrum cache: k1 / k1n keep the packed spectrum of every frame pair so k2 does not re-transform
     const int zpairs = (g.T + 1) / 2;
     const bool use_zcache = !generic && !(p.path_flags & 2);
@@ -1340,6 +1357,15 @@ int b200gate_run(b200gate_handle* h, const void* in, void* out, int dtype, int64
     // dual kernels (gate_dual.cuh): two channels of a chunk per warp -- stationary numpy-surface gate, even channel count.
     // Opt-in (path_flags bit 4): without packed FP32 instructions (sm_90) they are slower than one unit per warp.
     const bool use_dual = use_zcache && stat && !torch_sem && native && (C % 2 == 0) && (p.path_flags & 16);
+    // stationary mask smoothing inside k2c_synthesize (kMaskBits*) for every filter the byte-lane arithmetic holds; the
+    // separate smoothing kernel and the uint16 numerators in the workspace remain for the rest, for the dual and
+    // re-transforming synthesis kernels, and on request (path_flags bit 8)
+    const bool smooth_in_k2 = stat && use_zcache && !use_dual && !(p.path_flags & 256) &&
+                              packed_smoothing_fits(p.n_grad_freq, p.n_grad_time);
+    const size_t num_bytes = smooth_in_k2 ? 0 : (size_t)num_unit_stride(g.T) * 2;
+    const size_t per_unit_2pass = (stat ? (size_t)g.T * kFW * 4 + (size_t)kFPad * 4 + (size_t)kFW * 4 + num_bytes + 64
+                                        : 2 * (size_t)g.T * FP * 4 + 64) +
+                                  (stat && torch_sem ? (size_t)g.T * kFPad * 4 + 2 * (size_t)kFPad * 4 : 0) + 2048;
     // general-geometry family: float64 spectrum, mask, scratch and synthesis frames of every unit
     const size_t g_tf = (size_t)g.T * (size_t)h->F, g_tw = (size_t)g.T * (size_t)h->g_W;
     const size_t per_unit_generic = g_tf * 16 + 2 * g_tf * 8 + g_tw * 8 + 2 * (size_t)h->F * 8 + 6 * 256;
@@ -1413,7 +1439,7 @@ int b200gate_run(b200gate_handle* h, const void* in, void* out, int dtype, int64
     const size_t off_rowmax = off_bits + al((size_t)ub * g.T * kFW * 4);
     const size_t off_rowflag = off_rowmax + al((size_t)ub * kFPad * 4);
     const size_t off_num = off_rowflag + al((size_t)ub * kFW * 4);
-    const size_t end_stat = off_num + al((size_t)ub * num_unit_stride(g.T) * 2);
+    const size_t end_stat = off_num + al((size_t)ub * num_bytes);
     const size_t off_m0 = al((size_t)ub * g.T * FP * 4);
     const size_t end_nonstat = off_m0 + al((size_t)ub * g.T * FP * 4);
     // torch surface, stationary: the stationary buffers follow the dB spectrogram
@@ -1722,9 +1748,12 @@ int b200gate_run(b200gate_handle* h, const void* in, void* out, int dtype, int64
                 sa.n_units = nu; sa.T = g.T; sa.nf = nf; sa.nt = nt; sa.tf_lo = tf_lo; sa.tf_hi = tf_hi; sa.TT = 32;
                 sa.bits = d_bits; sa.rowflag = d_rowflag; sa.num = d_num;
                 const int ntaps = 2 * nf + 1;
-                if (h->reuse_masks) {
+                if (smooth_in_k2) {
+                    // k2c_synthesize smooths the decisions itself (they and the row flags stay in the workspace, so the
+                    // reuse_masks backward gets the forward's masks too)
+                } else if (h->reuse_masks) {
                     // the numerators of the last forward are still in d_num
-                } else if (nt + 1 <= 14 && ntaps <= 36) {
+                } else if (packed_smoothing_fits(nf, nt)) {
                     SmoothPArgs pa{};
                     pa.n_units = nu; pa.T = g.T; pa.nf = nf; pa.nt = nt; pa.tf_lo = tf_lo; pa.tf_hi = tf_hi;
                     pa.bits = d_bits; pa.rowflag = d_rowflag; pa.num = d_num;
@@ -1788,6 +1817,19 @@ int b200gate_run(b200gate_handle* h, const void* in, void* out, int dtype, int64
                         B200_WITH_DTYPE(kdt, { auto kern2 = k2d_synthesize<8, false, T>;
                             B200_LAUNCH(kern2, dim3(grid_1d(itemsd, kDualWarpsK2, h->num_sm)), dim3(kDualWarpsK2 * 32),
                                         k2d_smem_bytes(), st, ad); });
+                    }
+                } else if (smooth_in_k2) {         // cached spectra, smoothing of the decisions in the same kernel
+                    a2.num = nullptr;
+                    a2.bits = d_bits; a2.rowflag = d_rowflag;
+                    set_k2c_smoothing_taps(a2, nf);
+                    if (a2.one_minus_p != 0.f) {
+                        B200_WITH_DTYPE(kdt, { auto kern2 = k2c_synthesize<8, kMaskBitsBlend, T>;
+                            B200_LAUNCH(kern2, dim3(grid_1d(items2, kWarps, resident)), dim3(kThreads),
+                                        k2c_smem_bytes<kMaskBitsBlend>(), st, a2); });
+                    } else {
+                        B200_WITH_DTYPE(kdt, { auto kern2 = k2c_synthesize<8, kMaskBits, T>;
+                            B200_LAUNCH(kern2, dim3(grid_1d(items2, kWarps, resident)), dim3(kThreads),
+                                        k2c_smem_bytes<kMaskBits>(), st, a2); });
                     }
                 } else if (use_zcache) {           // spectra kept by k1: bulk-staged synthesis (gate_synth.cuh)
                     if (a2.one_minus_p != 0.f) {

@@ -709,6 +709,13 @@ struct K2Args {
     DebugTap dbg;
     const float2* zcache;          // optional: spectra stored by k1 / k1n (frames then are not re-transformed)
     int zpairs;
+    // k2c_synthesize kMaskBits*: smoothing inside synthesis (gate_synth.cuh) from the decisions instead of `num`
+    const unsigned* bits;          // [n_units][T][FW]
+    const unsigned* rowflag;       // [n_units][FW]
+    int sm_pad;                    // zero halo bytes before bin 0 of a time-sum row: nf rounded up to a multiple of 16
+    int sm_ws;                     // first tap word of bin group i: row word i + sm_ws
+    int sm_ntw;                    // tap words (4, 7, 9 or 10)
+    unsigned sm_taps[10];          // triangle taps nf+1-|d| as bytes, after (sm_pad - nf) % 4 zero bytes
 };
 
 constexpr int k2_smem_floats(int H) { return 2 * kN + 2 * kN + H + kFPad + kWarps * kExchFloats + 8 + kWarps * 2 * kN; }

@@ -9,7 +9,8 @@
 //   1. the pair's packed spectrum Z = X_a + i X_b (8 KB, written by k1 / k1n) and its two mask rows arrive in
 //      this warp's shared-memory buffers by 1-D bulk asynchronous copies (cp.async.bulk -> TMA engine, SASS
 //      UBLKCP) signalled on a per-warp mbarrier; the copies of pair t+2 are issued as soon as pair t has been
-//      read, so they travel behind a whole inverse transform;
+//      read, so they travel behind a whole inverse transform (kMaskBits*: only the spectrum is copied; the kernel
+//      smooths the pair's mask rows from the 1-bit decisions itself, see below);
 //   2. masks are applied on the packed spectrum,  Z'[k] = s Z[k] + d conj(Z[N-k]),  s, d = (m_a +- m_b)/2.
 //      The mirrored bin is read from the same shared buffer by its FLAT index (N - k) & (N - 1), which is what
 //      makes lane 0 (bins 0, 32, ... whose mirrors live in other SLOTS of the same lane) an ordinary lane: no
@@ -104,7 +105,18 @@ __device__ __forceinline__ unsigned prmt(unsigned a, unsigned b, unsigned sel) {
 #endif
 }
 
-enum { kMaskU16 = 0, kMaskU16Blend = 1, kMaskF32 = 2 };
+// Mask modes.  kMaskU16*: the pair's integer numerators are bulk-copied from `num` (written by k_smooth_packed /
+// k_smooth_generic).  kMaskBits*: the kernel smooths the mask itself from the 1-bit decisions (`bits` | `rowflag`),
+// with k_smooth_packed's integer arithmetic, so the numerators never leave shared memory:
+//   time direction   per-bin second-difference recurrence (triangle = box * box) in byte lanes, 4 bins per word;
+//                    a lane owns bins 16 lane .. 16 lane + 15 (one nibble of bits per 4 bins) and lane 0 also bins
+//                    512..515; the (d1, s2) state of the warp's unit lives in shared memory between pairs and is warmed
+//                    up from the 2 nt frames before the item's first pair;
+//   frequency        dp4a dot products of the time sums (two byte rows, one per frame, in the idle exchange tile) with
+//                    the packed triangle taps; the results go to `mbuf` in the num_index pair layout, which is what the
+//                    kMaskU16 modes would have copied there.
+// *Blend: prop_decrease < 1 (the edge-factor term of the zero-padded smoothing).
+enum { kMaskU16 = 0, kMaskU16Blend = 1, kMaskF32 = 2, kMaskBits = 3, kMaskBitsBlend = 4 };
 #ifndef B200_K2C_PTW
 #define B200_K2C_PTW 0              // inter-pass twiddles on packed register pairs (warp_fft1024_ptw)
 #endif
@@ -112,10 +124,53 @@ enum { kMaskU16 = 0, kMaskU16Blend = 1, kMaskF32 = 2 };
 
 constexpr int kK2cTableBytes = kN * 4 + kN * 8 + kFPad * 4;          // synthesis window, twiddles, frequency edge factors
 constexpr int kK2cTileBytes = kExchFloats * 4;                        // 4224: FFT exchange tile, also the 513 x float2 mirror buffer
-template <int MK> __host__ __device__ constexpr int k2c_mask_bytes() { return MK == kMaskF32 ? 2 * kFPad * 4 : 2 * kFPad * 2; }
+constexpr int kSynGroups = kF / 4 + 1;                                // 129 four-bin groups: bins 0..515
+constexpr int kSynNumBytes = kSynGroups * 16;                         // 2064: the pair's numerators, bins 0..515
+constexpr int kSynStateBytes = (kSynGroups * 8 + 15) & ~15;           // 1040: (d1, s2) per group
+constexpr int kSynRowPitch = 32 + 640;                                // time-sum row: <= 32 halo bytes + 160 groups of 4 bins
+constexpr int kSynMaxTapWords = 10;
+static_assert(2 * kSynRowPitch <= kK2cTileBytes, "time-sum rows must fit the exchange tile");
+template <int MK> __host__ __device__ constexpr int k2c_mask_bytes() {
+    return MK == kMaskF32 ? 2 * kFPad * 4 : (MK >= kMaskBits ? kSynNumBytes + kSynStateBytes : 2 * kFPad * 2);
+}
 template <int MK> __host__ __device__ constexpr int k2c_warp_bytes() { return kN * 8 + k2c_mask_bytes<MK>() + kK2cTileBytes + 16; }
 template <int MK> __host__ __device__ constexpr int k2c_smem_bytes() { return kK2cTableBytes + kWarps * k2c_warp_bytes<MK>(); }
 static_assert(kK2cTileBytes >= 513 * 8, "mirror buffer must fit the exchange tile");
+
+// kMaskBits*, frequency direction of one frame pair: rows = the two time-sum byte rows (row byte sm_pad + k = bin k),
+// num = the pair's numerators (num_index pair layout, bins 0..515).  Group i (bins 4i..4i+3) goes to lane i % 32, so
+// the row words a lane reads and the 16-byte results it stores are consecutive across the warp.
+template <int NTW>
+__device__ __forceinline__ void k2c_freq_taps(const unsigned char* rows, unsigned char* num, const K2Args& a, int lane) {
+    unsigned taps[NTW];
+#pragma unroll
+    for (int m = 0; m < NTW; ++m) taps[m] = a.sm_taps[m];
+#pragma unroll
+    for (int j = 0; j < 5; ++j) {
+        const int i = lane + 32 * j;
+        if (j == 4 && i >= kSynGroups) break;                  // the fifth group is lane 0's (bins 512..515)
+        unsigned o[2][4];
+#pragma unroll
+        for (int r = 0; r < 2; ++r) {
+            const unsigned* rw = reinterpret_cast<const unsigned*>(rows + r * kSynRowPitch) + i + a.sm_ws;
+            unsigned wv[NTW + 1];
+#pragma unroll
+            for (int m = 0; m <= NTW; ++m) wv[m] = rw[m];
+#pragma unroll
+            for (int jj = 0; jj < 4; ++jj) {
+                unsigned acc = 0u;
+#pragma unroll
+                for (int m = 0; m < NTW; ++m) {
+                    const unsigned win = (jj == 0) ? wv[m] : __funnelshift_r(wv[m], wv[m + 1], 8 * jj);
+                    acc = dp4a_u(win, taps[m], acc);
+                }
+                o[r][jj] = acc;
+            }
+        }
+        *reinterpret_cast<uint4*>(num + 16 * i) = uint4{o[0][0] | (o[1][0] << 16), o[0][1] | (o[1][1] << 16),
+                                                        o[0][2] | (o[1][2] << 16), o[0][3] | (o[1][3] << 16)};
+    }
+}
 
 #ifndef B200_K2C_MINBLOCKS
 #define B200_K2C_MINBLOCKS 3
@@ -125,6 +180,8 @@ __global__ void __launch_bounds__(kThreads, B200_K2C_MINBLOCKS) k2c_synthesize(c
     constexpr int NH = 32 / HR;             // frames overlapping one hop (win / hop)
     constexpr int MB = k2c_mask_bytes<MK>();
     constexpr int WB = k2c_warp_bytes<MK>();
+    constexpr bool kBits = MK == kMaskBits || MK == kMaskBitsBlend;                 // smoothing in this kernel
+    constexpr bool kBlend = MK == kMaskU16Blend || MK == kMaskBitsBlend;
     B200_DYN_SMEM(unsigned char, smraw);
     const Geom& g = a.g;
     const int H = g.H;
@@ -184,7 +241,7 @@ __global__ void __launch_bounds__(kThreads, B200_K2C_MINBLOCKS) k2c_synthesize(c
         const int t_last = min(he - 1, g.T - 1);
         T* yrow = static_cast<T*>(a.y) + (long long)c * g.out_stride;
         const float2* zunit = a.zcache + (long long)ul * a.zpairs * 1024;
-        const unsigned short* munit = (MK == kMaskF32) ? nullptr : a.num + (long long)ul * a.zpairs * (2 * kFPad);
+        const unsigned short* munit = (MK == kMaskF32 || kBits) ? nullptr : a.num + (long long)ul * a.zpairs * (2 * kFPad);
         const float* funit = (MK == kMaskF32) ? a.fmask + (long long)ul * g.T * kFPad : nullptr;
 
         float acc[32 + HR];
@@ -197,18 +254,99 @@ __global__ void __launch_bounds__(kThreads, B200_K2C_MINBLOCKS) k2c_synthesize(c
             __syncwarp();
             if (lane == 0) {
                 const bool vb2 = tt + 1 <= t_last;
-                const unsigned mbytes = (MK == kMaskF32 && !vb2) ? (unsigned)(kFPad * 4) : (unsigned)MB;
+                const unsigned mbytes = kBits ? 0u : ((MK == kMaskF32 && !vb2) ? (unsigned)(kFPad * 4) : (unsigned)MB);
                 mbar_expect_tx(bar, (unsigned)(kN * 8) + mbytes);
                 bulk_g2s(zbuf, zunit + (long long)(tt >> 1) * 1024, kN * 8, bar);
                 if (MK == kMaskF32) bulk_g2s(mbuf, funit + (long long)tt * kFPad, mbytes, bar);
-                else bulk_g2s(mbuf, munit + (long long)(tt >> 1) * (2 * kFPad), mbytes, bar);
+                else if (!kBits) bulk_g2s(mbuf, munit + (long long)(tt >> 1) * (2 * kFPad), mbytes, bar);
             }
         };
         if (t_start <= t_last) stage(t_start);
 
+        // ---- kMaskBits*: time-direction recurrence of k_smooth_packed, frames fed from tau_s = t_start - nt on ------
+        const int aa = a.nt + 1, tau_s = t_start - a.nt;
+        const unsigned* bunit = kBits ? a.bits + (long long)ul * g.T * kFW : nullptr;
+        uint2* sstate = reinterpret_cast<uint2*>(mbuf + kSynNumBytes);     // [4][32] lane groups, then group 128
+        // the top_db row flags of this lane's bins (x: its bits word, y: bins 512..515), OR-ed into every frame
+        auto rowflags = [&]() -> uint2 {
+            return uint2{__ldg(a.rowflag + ul * kFW + (lane >> 1)), __ldg(a.rowflag + ul * kFW + 16)};
+        };
+        // this lane's decisions of frame tau: x = its 16 bins (4 bits per group), y = bins 512..515 (lane 0 only);
+        // frames before tau_s count as zero, as in k_smooth_packed
+        auto fetch = [&](int tau, uint2 fl) -> uint2 {
+            if (tau < tau_s || tau < 0 || tau >= g.T) return uint2{0u, 0u};
+            const unsigned* row = bunit + (long long)tau * kFW;
+            const unsigned w = __ldg(row + (lane >> 1)) | fl.x;
+            const unsigned w5 = (__ldg(row + 16) | fl.y) & 0xFu;
+            return uint2{w >> ((lane & 1) * 16), lane == 0 ? w5 : 0u};
+        };
+        auto advance = [&](int tau, uint2 fl, unsigned (&d1)[5], unsigned (&s2)[5]) {
+            const uint2 na = fetch(tau, fl), nb = fetch(tau - aa, fl), nc = fetch(tau - 2 * aa, fl);
+#pragma unroll
+            for (int j = 0; j < 5; ++j) {
+                const unsigned xa = j < 4 ? na.x >> (4 * j) : na.y;
+                const unsigned xb = j < 4 ? nb.x >> (4 * j) : nb.y;
+                const unsigned xc = j < 4 ? nc.x >> (4 * j) : nc.y;
+                const unsigned ea = ((xa & 0xFu) * 0x00204081u) & 0x01010101u;         // nibble -> one bit per byte
+                const unsigned eb = ((xb & 0xFu) * 0x00204081u) & 0x01010101u;
+                const unsigned ec = ((xc & 0xFu) * 0x00204081u) & 0x01010101u;
+                d1[j] = d1[j] + ea + ec - 2u * eb;                                       // biased by 0x10 per byte
+                s2[j] = s2[j] + d1[j] - 0x10101010u;
+            }
+        };
+        auto save_state = [&](const unsigned (&d1)[5], const unsigned (&s2)[5]) {
+#pragma unroll
+            for (int j = 0; j < 4; ++j) sstate[32 * j + lane] = uint2{d1[j], s2[j]};
+            if (lane == 0) sstate[128] = uint2{d1[4], s2[4]};
+        };
+        if (kBits && t_start <= t_last) {               // warm-up: the 2 nt frames before the first pair's centre
+            unsigned d1[5], s2[5];
+#pragma unroll
+            for (int j = 0; j < 5; ++j) { d1[j] = 0x10101010u; s2[j] = 0u; }
+            const uint2 fl = rowflags();
+#pragma unroll 1
+            for (int tau = tau_s; tau < t_start + a.nt; ++tau) advance(tau, fl, d1, s2);
+            save_state(d1, s2);
+        }
+
         for (int t = t_start; t < he; t += 2) {
             const bool va = (t <= t_last), vb = (t + 1 <= t_last);
             if (va) {                                   // vb implies va
+                if (kBits) {                            // this pair's numerators, into mbuf
+                    unsigned d1[5], s2[5];
+#pragma unroll
+                    for (int j = 0; j < 4; ++j) {
+                        const uint2 v = sstate[32 * j + lane];
+                        d1[j] = v.x;
+                        s2[j] = v.y;
+                    }
+                    {
+                        const uint2 v = sstate[128];
+                        d1[4] = lane == 0 ? v.x : 0x10101010u;
+                        s2[4] = lane == 0 ? v.y : 0u;
+                    }
+                    const uint2 fl = rowflags();
+                    unsigned char* rows = reinterpret_cast<unsigned char*>(tile);
+                    __syncwarp();                       // the previous pair's transform is done with the tile
+#pragma unroll
+                    for (int r = 0; r < 2; ++r) {       // time sums of frames t, t+1 (centres of tau = t + nt, t + 1 + nt)
+                        advance(t + r + a.nt, fl, d1, s2);
+                        unsigned char* row = rows + r * kSynRowPitch;
+                        *reinterpret_cast<uint4*>(row + a.sm_pad + 16 * lane) = uint4{s2[0], s2[1], s2[2], s2[3]};
+                        // lane 0: bins 512..515; lanes 1..31: the zero tail the taps of the last bins read
+                        *reinterpret_cast<unsigned*>(row + a.sm_pad + 512 + 4 * lane) = s2[4];
+                        if (4 * lane < a.sm_pad) reinterpret_cast<unsigned*>(row)[lane] = 0u;     // zero halo
+                    }
+                    save_state(d1, s2);
+                    __syncwarp();
+                    switch (a.sm_ntw) {
+                        case 4: k2c_freq_taps<4>(rows, mbuf, a, lane); break;
+                        case 7: k2c_freq_taps<7>(rows, mbuf, a, lane); break;
+                        case 9: k2c_freq_taps<9>(rows, mbuf, a, lane); break;
+                        default: k2c_freq_taps<kSynMaxTapWords>(rows, mbuf, a, lane); break;
+                    }
+                    __syncwarp();                       // numerators visible; the tile is free for the mirror buffer
+                }
                 float re[32], im[32];                   // what the FFT call sees: re = Im Z', im = Re Z'
                 mbar_wait(bar, phase);
                 phase ^= 1u;
@@ -225,7 +363,7 @@ __global__ void __launch_bounds__(kThreads, B200_K2C_MINBLOCKS) k2c_synthesize(c
                     ca = -8388608.0f * pa;              // the 2^23 of the integer -> float bit pattern, folded into the FMA
                     pb = vb ? pa : 0.f;
                     cb = vb ? ca : 0.f;
-                    if (MK == kMaskU16Blend) {
+                    if (kBlend) {
                         eta = 0.5f * a.one_minus_p * time_edge(t, g.T, a.nt);
                         etb = vb ? 0.5f * a.one_minus_p * time_edge(t + 1, g.T, a.nt) : 0.f;
                     }
@@ -238,7 +376,7 @@ __global__ void __launch_bounds__(kThreads, B200_K2C_MINBLOCKS) k2c_synthesize(c
                         const unsigned pk = m32[kk];
                         const float fa = __uint_as_float(prmt(pk, 0x4B00u, 0x5410u));     // 2^23 + n_a
                         const float fb = __uint_as_float(prmt(pk, 0x4B00u, 0x5432u));     // 2^23 + n_b
-                        if (MK == kMaskU16Blend) {
+                        if (kBlend) {
                             const float e = s_ef[kk];
                             ma = fmaf(fa - 8388608.0f, pa, eta * e);
                             mb = fmaf(fb - 8388608.0f, pb, etb * e);
