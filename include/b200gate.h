@@ -67,15 +67,18 @@ typedef struct b200gate_params {
     int32_t path_flags;         /* kept cross-check variants of the same arithmetic (default 0).  bit 1: do not cache
                                  * spectra between analysis and synthesis (re-transform instead; saves 8 KB of workspace per
                                  * frame pair); bit 2: run the float64 general-geometry family even for a tuned geometry;
-                                 * bit 3: k1 streams the next frame pair's float32 sample rows into shared memory with
-                                 * cp.async (measured: no gain); bit 4: two units per warp in the n_fft 1024 FFT kernels
+                                 * bit 4: two units per warp in the n_fft 1024 FFT kernels
                                  * (the dual forms) instead of one; bit 5: tile-based float-mask smoothing;
                                  * bit 6: the non-stationary follower stores its forward sweep instead of regenerating
                                  * it; bit 7: tap-loop float-mask smoothing instead of the box-sum form; bit 8: stationary
                                  * gate, smooth the binary mask in a separate kernel that stores 16-bit numerators for the
                                  * synthesis kernel to read, instead of inside the synthesis kernel (same integers, more
-                                 * workspace and HBM traffic).  (bit 0 selected a single-pass experiment that was removed;
-                                 * it is ignored)                                                                      */
+                                 * workspace and HBM traffic); bit 9: stationary gate, n_fft 1024, one unit per warp: the
+                                 * analysis kernel that tracks the top_db row maxima of every bin and loads its samples
+                                 * directly does the whole analysis, instead of the kernel that prefetches sample windows
+                                 * by bulk copy and leaves the maxima to that kernel only when a frame could reach the
+                                 * floor (same arithmetic).  (bit 0 selected a single-pass experiment and bit 3 a
+                                 * cp.async staging of k1's sample rows; both were removed and are ignored)           */
     int64_t chunk_size;         /* <= 0: never chunk (torch surface / chunk_size=None)           */
     int64_t padding;
     double sr;

@@ -468,7 +468,7 @@ __global__ void __launch_bounds__(kDualWarpsK1 * 32, 1) k1d_analyze(const K1dArg
                             const int src = __ffs((int)m) - 1;
                             m &= m - 1;
                             const int r = recheck_bin_fp64(xrow, base + (long long)(uf & 1) * H, i1, g.Lp, g.n_total,
-                                                           src + 32 * q, a.tb, lane);
+                                                           src + 32 * q, a.tb.wa64, a.tb.cs64, a.tb.thr2_64, lane);
                             ++nre;
                             if (r == 0) { ++nun; continue; }
                             if (lane == q) {

@@ -911,6 +911,7 @@ int b200gate_create(const b200gate_params* p, b200gate_handle** out) {
         for (int dt = 0; dt < 3; ++dt)
             B200_WITH_DTYPE(dt, {
                 cudaFuncSetAttribute(k1_analyze<8, T>, cudaFuncAttributeMaxDynamicSharedMemorySize, k1_smem_floats() * 4);
+                cudaFuncSetAttribute(k1_analyze<8, T, true>, cudaFuncAttributeMaxDynamicSharedMemorySize, k1_smem_floats() * 4);
                 cudaFuncSetAttribute(k2_synthesize<8, false, T>, cudaFuncAttributeMaxDynamicSharedMemorySize, k2_smem_floats(256) * 4);
                 cudaFuncSetAttribute(k2_synthesize<8, true, T>, cudaFuncAttributeMaxDynamicSharedMemorySize, k2_smem_floats(256) * 4);
                 cudaFuncSetAttribute(k1n_magnitude<8, T>, cudaFuncAttributeMaxDynamicSharedMemorySize, k1n_smem_floats() * 4);
@@ -923,7 +924,6 @@ int b200gate_create(const b200gate_params* p, b200gate_handle** out) {
                 cudaFuncSetAttribute(k2c_synthesize<8, kMaskBits, T>, cudaFuncAttributeMaxDynamicSharedMemorySize, k2c_smem_bytes<kMaskBits>());
                 cudaFuncSetAttribute(k2c_synthesize<8, kMaskBitsBlend, T>, cudaFuncAttributeMaxDynamicSharedMemorySize, k2c_smem_bytes<kMaskBitsBlend>());
             });
-        cudaFuncSetAttribute(k1_analyze<8, float, true>, cudaFuncAttributeMaxDynamicSharedMemorySize, k1_smem_floats_staged() * 4);
         cudaFuncSetAttribute(k_smooth_f, cudaFuncAttributeMaxDynamicSharedMemorySize, 200 * 1024);
         cudaFuncSetAttribute(k_smooth_stream, cudaFuncAttributeMaxDynamicSharedMemorySize, 200 * 1024);
         for (int nfb = 1; nfb <= 12; ++nfb) smooth_box_dispatch(SmoothFArgs{}, nfb, dim3(1), 0, nullptr, true);
@@ -1692,7 +1692,6 @@ int b200gate_run(b200gate_handle* h, const void* in, void* out, int dtype, int64
                 a1.g = g; a1.tb = tb; a1.x = xb; a1.bits = d_bits; a1.rowmax = d_rowmax; a1.cnt = h->d_cnt; a1.dbg = dbg;
                 a1.zcache = d_zcache; a1.zpairs = zpairs;
                 a1.z_lo = tf_lo; a1.z_hi = tf_hi + 1;           // k2 walks pairs (2j, 2j+1) of frames [tf_lo, tf_hi)
-                a1.stage_rows = ((p.path_flags & 8) && kdt == B200GATE_F32) ? 1 : 0;
                 {
                     long long want = (long long)h->num_sm * B200_K1_MINBLOCKS * kWarps * 4;
                     long long run = ((long long)nu * g.T + want - 1) / want;
@@ -1702,10 +1701,13 @@ int b200gate_run(b200gate_handle* h, const void* in, void* out, int dtype, int64
                     a1.n_runs = (g.T + a1.run - 1) / a1.run;
                 }
                 const long long items1 = (long long)nu * a1.n_runs;
+                const unsigned grid1 = (unsigned)grid_1d(items1, kWarps, h->num_sm * B200_K1_MINBLOCKS);
+                // The analysis kernels below leave out the per-bin row maxima of the top_db floor and raise a device flag
+                // when a frame could reach the floor; the row-maximum kernel k1_analyze<.., true> then runs behind them
+                // (and returns at once otherwise).  path_flags bit 9: that kernel alone does the whole analysis.
+                CK(h, cudaMemsetAsync(h->d_need_rowmax, 0, sizeof(unsigned), st));
                 if (use_dual) {
-                    // two channels per warp (gate_dual.cuh); the single-unit kernel below runs only if a frame could
-                    // reach the top_db floor (device flag), to supply the per-bin row maxima
-                    CK(h, cudaMemsetAsync(h->d_need_rowmax, 0, sizeof(unsigned), st));
+                    // two channels per warp (gate_dual.cuh)
                     K1dArgs ad{};
                     ad.g = g; ad.tb = tb; ad.x = xb; ad.bits = d_bits; ad.zd = (float4*)d_zcache; ad.zpairs = zpairs;
                     ad.z_lo = tf_lo; ad.z_hi = tf_hi + 1; ad.cnt = h->d_cnt; ad.need_rowmax = h->d_need_rowmax;
@@ -1726,16 +1728,17 @@ int b200gate_run(b200gate_handle* h, const void* in, void* out, int dtype, int64
                     ++launches;
                     a1.guard = h->d_need_rowmax;
                     a1.zcache = nullptr;
-                }
-                if (a1.stage_rows) {
-                    auto kern_ = k1_analyze<8, float, true>;
-                    B200_LAUNCH(kern_, dim3(grid_1d(items1, kWarps, h->num_sm * B200_K1_MINBLOCKS)), dim3(kThreads),
-                                k1_smem_floats_staged() * 4, st, a1);
-                } else {
+                } else if (!(p.path_flags & 512)) {
+                    a1.need_rowmax = h->d_need_rowmax;
+                    a1.min_floor4 = (float)(4.0 * h->min_floor_amp * h->min_floor_amp);
                     B200_WITH_DTYPE(kdt, { auto kern_ = k1_analyze<8, T>;
-                        B200_LAUNCH(kern_, dim3(grid_1d(items1, kWarps, h->num_sm * B200_K1_MINBLOCKS)), dim3(kThreads),
-                                    k1_smem_floats() * 4, st, a1); });
+                        B200_LAUNCH(kern_, dim3(grid1), dim3(kThreads), k1_smem_floats() * 4, st, a1); });
+                    ++launches;
+                    a1.guard = h->d_need_rowmax;
+                    a1.zcache = nullptr;
                 }
+                B200_WITH_DTYPE(kdt, { auto kern_ = k1_analyze<8, T, true>;
+                    B200_LAUNCH(kern_, dim3(grid1), dim3(kThreads), k1_smem_floats() * 4, st, a1); });
                 B200_LAUNCH(k_rowfloor, dim3(grid_1d((long long)nu * kFW, 256, 1 << 30)), dim3(256), 0, st, nu,
                             (const unsigned*)d_rowmax, (const float*)h->d_floor4, d_rowflag, h->d_cnt);
             }

@@ -165,10 +165,8 @@ __device__ __forceinline__ float pack_frame_pair(float (&re)[32], float (&im)[32
 }
 
 template <int HR, typename T>
-__device__ __forceinline__ float load_frame_pair(float (&re)[32], float (&im)[32], const T* __restrict__ xrow,
-                                                 long long base, long long i1, long long Lp, long long n_total,
-                                                 const float* __restrict__ s_wa, int lane, bool vb) {
-    float xr[32 + HR];
+__device__ __forceinline__ void load_pair_rows(float (&xr)[32 + HR], const T* __restrict__ xrow, long long base,
+                                               long long i1, long long Lp, long long n_total, int lane) {
     if (pair_window_interior<HR>(base, i1, Lp, n_total)) {
         const T* p = xrow + i1 + base + lane;
 #pragma unroll
@@ -177,6 +175,14 @@ __device__ __forceinline__ float load_frame_pair(float (&re)[32], float (&im)[32
 #pragma unroll
         for (int r = 0; r < 32 + HR; ++r) xr[r] = chunk_sample(xrow, base + lane + 32 * r, i1, Lp, n_total);
     }
+}
+
+template <int HR, typename T>
+__device__ __forceinline__ float load_frame_pair(float (&re)[32], float (&im)[32], const T* __restrict__ xrow,
+                                                 long long base, long long i1, long long Lp, long long n_total,
+                                                 const float* __restrict__ s_wa, int lane, bool vb) {
+    float xr[32 + HR];
+    load_pair_rows<HR>(xr, xrow, base, i1, Lp, n_total, lane);
     return pack_frame_pair<HR>(re, im, xr, s_wa, lane, vb);
 }
 
@@ -188,14 +194,6 @@ __device__ __forceinline__ void cp_async16(void* smem_dst, const void* gmem_src)
 #else
     const unsigned sa = (unsigned)__cvta_generic_to_shared(smem_dst);
     asm volatile("cp.async.cg.shared.global [%0], [%1], 16;" ::"r"(sa), "l"(gmem_src));
-#endif
-}
-__device__ __forceinline__ void cp_async4(void* smem_dst, const void* gmem_src) {
-#ifdef B200_CUSIM_BUILD
-    memcpy(smem_dst, gmem_src, 4);
-#else
-    const unsigned sa = (unsigned)__cvta_generic_to_shared(smem_dst);
-    asm volatile("cp.async.ca.shared.global [%0], [%1], 4;" ::"r"(sa), "l"(gmem_src));
 #endif
 }
 __device__ __forceinline__ void cp_async_commit_wait_all() {
@@ -214,6 +212,78 @@ __device__ __forceinline__ void cp_async_wait_all() {
 #endif
 }
 
+// ---- mbarrier + bulk asynchronous copy (global -> shared through the TMA engine) ------------------------------
+__device__ __forceinline__ void mbar_init(unsigned long long* bar, unsigned count) {
+#ifdef B200_CUSIM_BUILD
+    *bar = 0; (void)count;
+#else
+    const unsigned a = (unsigned)__cvta_generic_to_shared(bar);
+    asm volatile("mbarrier.init.shared::cta.b64 [%0], %1;" ::"r"(a), "r"(count) : "memory");
+#endif
+}
+__device__ __forceinline__ void mbar_init_fence() {
+#ifndef B200_CUSIM_BUILD
+    asm volatile("fence.mbarrier_init.release.cluster;" ::: "memory");
+#endif
+}
+__device__ __forceinline__ void mbar_expect_tx(unsigned long long* bar, unsigned bytes) {
+#ifdef B200_CUSIM_BUILD
+    (void)bar; (void)bytes;
+#else
+    const unsigned a = (unsigned)__cvta_generic_to_shared(bar);
+    asm volatile("mbarrier.arrive.expect_tx.shared::cta.b64 _, [%0], %1;" ::"r"(a), "r"(bytes) : "memory");
+#endif
+}
+// dst, src 16-byte aligned, bytes a multiple of 16
+__device__ __forceinline__ void bulk_g2s(void* smem_dst, const void* gmem_src, unsigned bytes, unsigned long long* bar) {
+#ifdef B200_CUSIM_BUILD
+    memcpy(smem_dst, gmem_src, bytes); (void)bar;
+#else
+    const unsigned d = (unsigned)__cvta_generic_to_shared(smem_dst);
+    const unsigned b = (unsigned)__cvta_generic_to_shared(bar);
+    asm volatile("cp.async.bulk.shared::cluster.global.mbarrier::complete_tx::bytes [%0], [%1], %2, [%3];"
+                 ::"r"(d), "l"(gmem_src), "r"(bytes), "r"(b) : "memory");
+#endif
+}
+__device__ __forceinline__ void mbar_wait(unsigned long long* bar, unsigned parity) {
+#ifdef B200_CUSIM_BUILD
+    (void)bar; (void)parity;
+    __syncwarp();                  // simulator: the issuing lane's (synchronous) copy precedes its own wait
+#else
+    const unsigned a = (unsigned)__cvta_generic_to_shared(bar);
+    asm volatile(
+        "{\n\t.reg .pred p;\n\t"
+        "W_%=:\n\t"
+        "mbarrier.try_wait.parity.shared::cta.b64 p, [%0], %1;\n\t"
+        "@p bra D_%=;\n\t"
+        "bra W_%=;\n\t"
+        "D_%=:\n\t}"
+        ::"r"(a), "r"(parity) : "memory");
+#endif
+}
+// order this thread's earlier generic-proxy accesses of shared memory before later async-proxy (bulk copy) writes
+__device__ __forceinline__ void fence_proxy_async_smem() {
+#ifndef B200_CUSIM_BUILD
+    asm volatile("fence.proxy.async.shared::cta;" ::: "memory");
+#endif
+}
+// shared -> global bulk copy (TMA store engine) of `bytes` (16-byte multiple, both sides 16-byte aligned); completion is
+// tracked by bulk groups: commit, then wait_group.read before the shared source is overwritten
+__device__ __forceinline__ void bulk_s2g(void* gmem_dst, const void* smem_src, unsigned bytes) {
+#ifdef B200_CUSIM_BUILD
+    memcpy(gmem_dst, smem_src, bytes);
+#else
+    const unsigned s = (unsigned)__cvta_generic_to_shared(smem_src);
+    asm volatile("cp.async.bulk.global.shared::cta.bulk_group [%0], [%1], %2;" ::"l"(gmem_dst), "r"(s), "r"(bytes) : "memory");
+    asm volatile("cp.async.bulk.commit_group;" ::: "memory");
+#endif
+}
+__device__ __forceinline__ void bulk_wait_read_all() {
+#ifndef B200_CUSIM_BUILD
+    asm volatile("cp.async.bulk.wait_group.read 0;" ::: "memory");
+#endif
+}
+
 #ifdef B200_CUSIM_BUILD
 #define B200_NOINLINE __attribute__((noinline))
 #else
@@ -222,21 +292,24 @@ __device__ __forceinline__ void cp_async_wait_all() {
 
 // Exact (float64) re-decision of one bin of one frame: direct DFT of the windowed samples.
 // Warp-cooperative; every lane returns the same value.  2 = above threshold, 1 = not above,
-// 0 = unresolved even in float64 (|P - T^2| <= 1e-12 T^2).
+// 0 = unresolved even in float64 (|P - T^2| <= 1e-12 T^2).  The tables come as pointers, not as `const Tables&`: a
+// reference into the kernel's parameters would make the caller copy them all to local memory.
 template <typename T>
 __device__ B200_NOINLINE int recheck_bin_fp64(const T* __restrict__ xrow, long long base, long long i1,
-                                              long long Lp, long long n_total, int k, const Tables& tb, int lane) {
+                                              long long Lp, long long n_total, int k, const double* __restrict__ wa64,
+                                              const double2* __restrict__ cs64, const double* __restrict__ thr2_64,
+                                              int lane) {
     double sr = 0.0, si = 0.0;
     for (int n = lane; n < kN; n += 32) {
-        const double x = chunk_sample_f64(xrow, base + n, i1, Lp, n_total) * tb.wa64[n];   // the caller's exact samples
-        const double2 cs = tb.cs64[(k * n) & (kN - 1)];
+        const double x = chunk_sample_f64(xrow, base + n, i1, Lp, n_total) * wa64[n];   // the caller's exact samples
+        const double2 cs = cs64[(k * n) & (kN - 1)];
         sr = fma(x, cs.x, sr);
         si = fma(-x, cs.y, si);
     }
     sr = warp_sum(sr);
     si = warp_sum(si);
     const double P = sr * sr + si * si;
-    const double T2 = tb.thr2_64[k];
+    const double T2 = thr2_64[k];
     if (fabs(P - T2) <= 1e-12 * T2) return 0;
     return P > T2 ? 2 : 1;
 }
@@ -249,7 +322,8 @@ struct K1Args {
     Tables tb;
     const void* x;             // [C][in_stride] samples in the caller's dtype (kernel template T)
     unsigned* bits;            // [n_units][T][FW]
-    unsigned* rowmax;          // [n_units][FPad]  max_t 4|X|^2 as float bits (>= 0 so uint order works)
+    unsigned* rowmax;          // [n_units][FPad]  max_t 4|X|^2 as float bits (>= 0 so uint order works); written only by
+                               // the row-maximum instantiation k1_analyze<.., true>
     Counters* cnt;
     DebugTap dbg;
     int run;                   // frames per work item (even)
@@ -259,17 +333,26 @@ struct K1Args {
     int zpairs;                // ceil(T/2)
     int z_lo, z_hi;            // only frames [z_lo, z_hi) are read back by k2 (chunk centre + halo): the rest is not stored
     const unsigned* guard;     // optional device flag: when given and zero the kernel returns at once (it is then the
-                               // row-maximum fallback behind k1d_analyze, gate_dual.cuh)
-    int stage_rows;            // set for the k1_analyze<.., true> instantiation (path_flags bit 3, float32 rows): the NEXT
-                               // pair's sample rows stream into shared memory (cp.async) behind the current pair's transform
+                               // row-maximum fallback behind k1_analyze<.., false> or k1d_analyze, gate_dual.cuh)
+    unsigned* need_rowmax;     // k1_analyze<.., false>: device flag raised when a frame could reach its top_db floor
+    float min_floor4;          // min over bins of 4 * (10^((thresh + top_db)/20) - eps)^2
 };
 
-constexpr int k1_smem_floats() { return kN + 2 * kN + 2 * kFPad + kWarps * kExchFloats + kWarps * 2 * kFW + 8; }
-constexpr int kStageFloats = 32 * (32 + 8);          // one pair's rows: 40 x 32 samples
-constexpr int k1_smem_floats_staged() { return k1_smem_floats() + kWarps * kStageFloats; }
+// One pair's sample window (32 + 8 rows of 32 samples) as the 16-byte-aligned span that covers it: up to 16 bytes more.
+constexpr int kK1WinBytes = 32 * (32 + 8) * 4 + 16;
+constexpr int k1_smem_floats() {
+    return kN + 2 * kN + 2 * kFPad + kWarps * kExchFloats + kWarps * 2 * kFW + 8 + kWarps * (kK1WinBytes / 4) + 2 * kWarps;
+}
 
-template <int HR, typename T, bool STAGE = false>
+// ROWMAX = false (default): the window of the warp's next frame pair streams into a per-warp shared buffer by one bulk
+// copy (TMA engine) while the current pair is transformed, and the top_db row maxima are not tracked: the kernel only
+// raises need_rowmax when a pair's energy could reach the lowest floor (|X_k|^2 <= N ||frame||^2), and the host then runs
+// the ROWMAX = true instantiation behind it (guarded by that flag) for the maxima.  That instantiation loads the samples
+// directly and tracks the maxima of every bin; run alone it is the whole analysis.
+template <int HR, typename T, bool ROWMAX = false>
 __global__ void __launch_bounds__(kThreads, B200_K1_MINBLOCKS) k1_analyze(const K1Args a) {
+    static_assert(32 * (32 + HR) * 4 + 16 <= kK1WinBytes, "sample window must fit the buffer");
+    constexpr bool kBulk = !ROWMAX && sizeof(T) <= 4;   // float32 / int16 windows (float64: direct loads)
     if (a.guard && *a.guard == 0u) return;
     B200_DYN_SMEM(float, smem);
     float* s_wa = smem;
@@ -278,7 +361,8 @@ __global__ void __launch_bounds__(kThreads, B200_K1_MINBLOCKS) k1_analyze(const 
     float* s_gco = s_thr4 + kFPad;
     float* s_tiles = s_gco + kFPad;
     unsigned* s_amb_all = reinterpret_cast<unsigned*>(s_tiles + kWarps * kExchFloats);
-    float* s_stage_all = reinterpret_cast<float*>(s_amb_all + kWarps * 2 * kFW + 8);    // only when a.stage_rows
+    unsigned char* s_win_all = reinterpret_cast<unsigned char*>(s_amb_all + kWarps * 2 * kFW + 8);   // 16-byte aligned
+    unsigned long long* s_bar_all = reinterpret_cast<unsigned long long*>(s_win_all + kWarps * kK1WinBytes);
     for (int i = threadIdx.x; i < kN; i += kThreads) {
         s_wa[i] = a.tb.wa[i];
         s_tw[i] = a.tb.tw[i];
@@ -287,70 +371,111 @@ __global__ void __launch_bounds__(kThreads, B200_K1_MINBLOCKS) k1_analyze(const 
         s_thr4[i] = a.tb.thr4[i];
         s_gco[i] = a.tb.gco[i];
     }
-    __syncthreads();
-
     const Geom& g = a.g;
     const int lane = threadIdx.x & 31, warp = threadIdx.x >> 5;
+    unsigned char* win = s_win_all + warp * kK1WinBytes;
+    unsigned long long* bar = s_bar_all + warp;
+    if (kBulk) {
+        if (lane == 0) mbar_init(bar, 1);
+        mbar_init_fence();
+    }
+    __syncthreads();
+    unsigned phase = 0;
+
     float* tile = s_tiles + warp * kExchFloats;
     unsigned* s_amb = s_amb_all + warp * 2 * kFW;
     const int H = g.H;
     const int pl = (32 - lane) & 31;                 // partner lane holding the mirrored bins
     const long long n_items = (long long)g.n_units * a.n_runs;
-
-    for (long long item = (long long)blockIdx.x * kWarps + warp; item < n_items;
-         item += (long long)gridDim.x * kWarps) {
-        const int ul = (int)(item / a.n_runs);
-        const int run = (int)(item - (long long)ul * a.n_runs);
-        const int u = g.u0 + ul;
+    const long long item_stride = (long long)gridDim.x * kWarps;
+    // work item = (local unit, run); the warp's items advance by item_stride = (step_ul, step_run) without dividing
+    const int step_ul = (int)(item_stride / a.n_runs), step_run = (int)(item_stride - (long long)step_ul * a.n_runs);
+    auto next_item = [&](int& ul_, int& run_) {
+        ul_ += step_ul;
+        run_ += step_run;
+        if (run_ >= a.n_runs) { run_ -= a.n_runs; ++ul_; }
+    };
+    // sample row and chunk origin (global index of chunk sample 0) of a local unit
+    auto unit_row = [&](int ul_, const T*& xrow, long long& i1) {
+        const int u = g.u0 + ul_;
         const int ic = u / g.C, c = u - ic * g.C;
-        const long long i1 = (long long)ic * g.step - g.pad;
-        const T* xrow = static_cast<const T*>(a.x) + (long long)c * g.in_stride;
+        i1 = (long long)ic * g.step - g.pad;
+        xrow = static_cast<const T*>(a.x) + (long long)c * g.in_stride;
+    };
+    // Request the window of pair (tt, tt + 1) of a unit into this warp's buffer when it lies inside the chunk and the
+    // recording and the 16-byte-aligned span covering it lies inside the row.  Returns the window's element offset in
+    // the buffer, or -1: the pair is then loaded directly.  Warp-uniform; every lane has finished reading the buffer.
+    auto request = [&](const T* xr_, long long i1_, int tt) -> int {
+        if (!kBulk) return -1;
+        const long long bb = (long long)tt * H - kN / 2;
+        if (!pair_window_interior<HR>(bb, i1_, g.Lp, g.n_total)) return -1;
+        const unsigned long long src = reinterpret_cast<unsigned long long>(xr_ + i1_ + bb);
+        const unsigned long long lo = src & ~15ull;
+        const unsigned long long hi = (src + 32 * (32 + HR) * sizeof(T) + 15) & ~15ull;
+        if (lo < reinterpret_cast<unsigned long long>(xr_) || hi > reinterpret_cast<unsigned long long>(xr_ + g.n_total))
+            return -1;
+        fence_proxy_async_smem();
+        __syncwarp();
+        if (lane == 0) {
+            mbar_expect_tx(bar, (unsigned)(hi - lo));
+            bulk_g2s(win, reinterpret_cast<const void*>(lo), (unsigned)(hi - lo), bar);
+        }
+        return (int)((src - lo) / sizeof(T));
+    };
+    long long item = (long long)blockIdx.x * kWarps + warp;
+    int ul = (int)(item / a.n_runs), run = (int)(item - (long long)ul * a.n_runs);
+    int woff = -1;                                   // element offset of the pending window in `win`, -1: none
+    if (kBulk && item < n_items) {
+        const T* xr_;
+        long long i1_;
+        unit_row(ul, xr_, i1_);
+        woff = request(xr_, i1_, run * a.run);
+    }
+
+    for (; item < n_items; item += item_stride, next_item(ul, run)) {
+        const T* xrow;
+        long long i1;
+        unit_row(ul, xrow, i1);
         const int t0 = run * a.run;
         const int t1 = min(t0 + a.run, g.T);
-        float mx[kFW];
+        float mx[ROWMAX ? kFW : 1];
+        if (ROWMAX) {
 #pragma unroll
-        for (int q = 0; q < kFW; ++q) mx[q] = 0.f;
-
-        // staged rows: request pair t's 40 rows (float32, interior of the chunk and the recording) into this
-        // warp's 5 KB buffer; 16-byte copies when the first row is 16-byte aligned, else one word per lane and row
-        float* sbuf = s_stage_all + warp * kStageFloats;
-        auto stage_rows = [&](int tt) -> bool {
-            if (!STAGE || sizeof(T) != 4) return false;       // compile-time: the default instantiation carries none of this
-            const long long bb = (long long)tt * H - kN / 2;
-            if (!pair_window_interior<HR>(bb, i1, g.Lp, g.n_total)) return false;
-            const char* src = reinterpret_cast<const char*>(xrow + i1 + bb);
-            char* dst = reinterpret_cast<char*>(sbuf);
-            if ((reinterpret_cast<unsigned long long>(src) & 15ull) == 0) {
-#pragma unroll
-                for (int j = 0; j < (32 + HR) / 4; ++j) cp_async16(dst + (lane + 32 * j) * 16, src + (lane + 32 * j) * 16);
-            } else {
-#pragma unroll
-                for (int r = 0; r < 32 + HR; ++r) cp_async4(dst + (lane + 32 * r) * 4, src + (lane + 32 * r) * 4);
-            }
-            cp_async_commit();
-            return true;
-        };
-        bool staged = STAGE && stage_rows(t0);
+            for (int q = 0; q < kFW; ++q) mx[q] = 0.f;
+        }
+        float emax = 0.f;                            // largest pair energy of the item (row floor test)
 
         for (int t = t0; t < t1; t += 2) {
             const bool vb = (t + 1 < t1);
             const long long base = (long long)t * H - kN / 2;
-            float re[32], im[32];
-            float e;
-            if (STAGE && staged) {                            // warp-uniform
-                float xr[32 + HR];
-                cp_async_wait_all();
-                __syncwarp();
+            float xr[32 + HR];
+            if (kBulk && woff >= 0) {                        // warp-uniform
+                mbar_wait(bar, phase);
+                phase ^= 1u;
+                const T* wp = reinterpret_cast<const T*>(win) + woff + lane;
 #pragma unroll
-                for (int r = 0; r < 32 + HR; ++r) xr[r] = sbuf[32 * r + lane];
-                __syncwarp();
-                staged = (t + 2 < t1) && stage_rows(t + 2);   // the next pair streams in behind this pair's transform
-                e = pack_frame_pair<HR>(re, im, xr, s_wa, lane, vb);
+                for (int r = 0; r < 32 + HR; ++r) xr[r] = (float)wp[32 * r];
             } else {
-                if (STAGE) staged = (t + 2 < t1) && stage_rows(t + 2);
-                e = load_frame_pair<HR>(re, im, xrow, base, i1, g.Lp, g.n_total, s_wa, lane, vb);
+                load_pair_rows<HR>(xr, xrow, base, i1, g.Lp, g.n_total, lane);
             }
-            const float S = sqrtf(warp_sum(e));
+            if (kBulk) {                                     // the next window streams in behind this pair's transform
+                if (t + 2 < t1) {
+                    woff = request(xrow, i1, t + 2);
+                } else if (item + item_stride < n_items) {   // the first window of the warp's next work item
+                    int uln = ul, runn = run;
+                    next_item(uln, runn);
+                    const T* xr_;
+                    long long i1_;
+                    unit_row(uln, xr_, i1_);
+                    woff = request(xr_, i1_, runn * a.run);
+                } else {
+                    woff = -1;
+                }
+            }
+            float re[32], im[32];
+            const float E = warp_sum(pack_frame_pair<HR>(re, im, xr, s_wa, lane, vb));
+            if (!ROWMAX) emax = fmaxf(emax, E);
+            const float S = sqrtf(E);
             warp_fft1024(re, im, tile, s_tw, lane);
             if (a.zcache && t >= a.z_lo && t < a.z_hi) {      // warp-uniform
                 float2* zp = a.zcache + ((long long)ul * a.zpairs + (t >> 1)) * 1024 + lane;
@@ -387,7 +512,7 @@ __global__ void __launch_bounds__(kThreads, B200_K1_MINBLOCKS) k1_analyze(const 
                     anyamb |= 1u << q;
                     if (lane == 0) { s_amb[2 * q] = mA; s_amb[2 * q + 1] = mB; }
                 }
-                if (valid) mx[q] = fmaxf(mx[q], vb ? fmaxf(PA, PB) : PA);
+                if (ROWMAX && valid) mx[q] = fmaxf(mx[q], vb ? fmaxf(PA, PB) : PA);
             }
             if (a.dbg.ul == ul) {                            // parity tap (tests): the FP32 STFT itself
 #pragma unroll 1
@@ -420,7 +545,7 @@ __global__ void __launch_bounds__(kThreads, B200_K1_MINBLOCKS) k1_analyze(const 
                             const int src = __ffs((int)m) - 1;
                             m &= m - 1;
                             const int r = recheck_bin_fp64(xrow, base + (long long)fr * H, i1, g.Lp, g.n_total,
-                                                           src + 32 * q, a.tb, lane);
+                                                           src + 32 * q, a.tb.wa64, a.tb.cs64, a.tb.thr2_64, lane);
                             ++nre;
                             if (r == 0) { ++nun; continue; }
                             if (lane == q) {
@@ -431,7 +556,7 @@ __global__ void __launch_bounds__(kThreads, B200_K1_MINBLOCKS) k1_analyze(const 
                     }
                 }
                 __syncwarp();
-                if (lane == 0) {
+                if (lane == 0 && !a.guard) {          // (a guarded fallback re-derives bins the kernel before it counted)
                     atomicAdd(&a.cnt->rechecked, (unsigned long long)nre);
                     if (nun) atomicAdd(&a.cnt->unresolved, (unsigned long long)nun);
                 }
@@ -442,10 +567,14 @@ __global__ void __launch_bounds__(kThreads, B200_K1_MINBLOCKS) k1_analyze(const 
                 if (vb) dst[kFW] = wordB;
             }
         }
+        if (ROWMAX) {
 #pragma unroll
-        for (int q = 0; q < kFW; ++q)
-            if ((q < 16) || (lane == 0))
-                atomicMax(a.rowmax + (long long)ul * kFPad + lane + 32 * q, __float_as_uint(mx[q]));
+            for (int q = 0; q < kFW; ++q)
+                if ((q < 16) || (lane == 0))
+                    atomicMax(a.rowmax + (long long)ul * kFPad + lane + 32 * q, __float_as_uint(mx[q]));
+        } else if (4.0f * (float)kN * emax >= 0.999f * a.min_floor4 && lane == 0) {
+            atomicOr(a.need_rowmax, 1u);             // |X|^2 <= N * (frame energy): a bin could reach its top_db floor
+        }
     }
 }
 

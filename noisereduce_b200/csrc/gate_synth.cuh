@@ -23,77 +23,6 @@
 
 namespace b200 {
 
-// ---- mbarrier + bulk asynchronous copy (global -> shared through the TMA engine) ------------------------------
-__device__ __forceinline__ void mbar_init(unsigned long long* bar, unsigned count) {
-#ifdef B200_CUSIM_BUILD
-    *bar = 0; (void)count;
-#else
-    const unsigned a = (unsigned)__cvta_generic_to_shared(bar);
-    asm volatile("mbarrier.init.shared::cta.b64 [%0], %1;" ::"r"(a), "r"(count) : "memory");
-#endif
-}
-__device__ __forceinline__ void mbar_init_fence() {
-#ifndef B200_CUSIM_BUILD
-    asm volatile("fence.mbarrier_init.release.cluster;" ::: "memory");
-#endif
-}
-__device__ __forceinline__ void mbar_expect_tx(unsigned long long* bar, unsigned bytes) {
-#ifdef B200_CUSIM_BUILD
-    (void)bar; (void)bytes;
-#else
-    const unsigned a = (unsigned)__cvta_generic_to_shared(bar);
-    asm volatile("mbarrier.arrive.expect_tx.shared::cta.b64 _, [%0], %1;" ::"r"(a), "r"(bytes) : "memory");
-#endif
-}
-// dst, src 16-byte aligned, bytes a multiple of 16
-__device__ __forceinline__ void bulk_g2s(void* smem_dst, const void* gmem_src, unsigned bytes, unsigned long long* bar) {
-#ifdef B200_CUSIM_BUILD
-    memcpy(smem_dst, gmem_src, bytes); (void)bar;
-#else
-    const unsigned d = (unsigned)__cvta_generic_to_shared(smem_dst);
-    const unsigned b = (unsigned)__cvta_generic_to_shared(bar);
-    asm volatile("cp.async.bulk.shared::cluster.global.mbarrier::complete_tx::bytes [%0], [%1], %2, [%3];"
-                 ::"r"(d), "l"(gmem_src), "r"(bytes), "r"(b) : "memory");
-#endif
-}
-__device__ __forceinline__ void mbar_wait(unsigned long long* bar, unsigned parity) {
-#ifdef B200_CUSIM_BUILD
-    (void)bar; (void)parity;
-    __syncwarp();                  // simulator: the issuing lane's (synchronous) copy precedes its own wait
-#else
-    const unsigned a = (unsigned)__cvta_generic_to_shared(bar);
-    asm volatile(
-        "{\n\t.reg .pred p;\n\t"
-        "W_%=:\n\t"
-        "mbarrier.try_wait.parity.shared::cta.b64 p, [%0], %1;\n\t"
-        "@p bra D_%=;\n\t"
-        "bra W_%=;\n\t"
-        "D_%=:\n\t}"
-        ::"r"(a), "r"(parity) : "memory");
-#endif
-}
-// order this thread's earlier generic-proxy accesses of shared memory before later async-proxy (bulk copy) writes
-__device__ __forceinline__ void fence_proxy_async_smem() {
-#ifndef B200_CUSIM_BUILD
-    asm volatile("fence.proxy.async.shared::cta;" ::: "memory");
-#endif
-}
-// shared -> global bulk copy (TMA store engine) of `bytes` (16-byte multiple, both sides 16-byte aligned); completion is
-// tracked by bulk groups: commit, then wait_group.read before the shared source is overwritten
-__device__ __forceinline__ void bulk_s2g(void* gmem_dst, const void* smem_src, unsigned bytes) {
-#ifdef B200_CUSIM_BUILD
-    memcpy(gmem_dst, smem_src, bytes);
-#else
-    const unsigned s = (unsigned)__cvta_generic_to_shared(smem_src);
-    asm volatile("cp.async.bulk.global.shared::cta.bulk_group [%0], [%1], %2;" ::"l"(gmem_dst), "r"(s), "r"(bytes) : "memory");
-    asm volatile("cp.async.bulk.commit_group;" ::: "memory");
-#endif
-}
-__device__ __forceinline__ void bulk_wait_read_all() {
-#ifndef B200_CUSIM_BUILD
-    asm volatile("cp.async.bulk.wait_group.read 0;" ::: "memory");
-#endif
-}
 __device__ __forceinline__ unsigned prmt(unsigned a, unsigned b, unsigned sel) {
 #ifdef B200_CUSIM_BUILD
     const unsigned long long v = ((unsigned long long)b << 32) | a;
