@@ -13,6 +13,8 @@
  *                                 nonstationary.py:47-115), i.e. the body of reduce_noise()
  *                                 (noisereduce/noisereduce.py:185), and TorchGate.forward
  *                                 (torchgate.py:200-264) when params.surface == B200GATE_SURFACE_TORCH
+ *   b200gate_stream_*          <- the same chunk loop on a recording that arrives block by block, in place of
+ *                                 the temp-file memmap the result is written to (base.py:181-187)
  *
  * Conventions: plain pointers and sizes, no torch / numpy types.  All buffers are caller-owned; the
  * library owns only its handle and device workspace.  Every function returns B200GATE_OK (0) or a
@@ -165,6 +167,33 @@ int b200gate_run(b200gate_handle* h, const void* in, void* out, int dtype, int64
  * may pass `slab - first_sample` with out_stride = the slab's row pitch (>= the range length) to have the range
  * written densely into a [C][range] slab (noisereduce_b200/parallel.py gathers such slabs across GPUs). */
 int b200gate_set_range(b200gate_handle* h, int32_t mode, int64_t a, int64_t b);
+
+/* ---- streaming: a recording that arrives block by block (numpy surface, chunk_size > 0) ----------------------------
+ * The reference holds the whole [C][N] input and writes the result to a temp-file memmap (base.py:181-187).  A stream
+ * returns each chunk as soon as its padded span has arrived, and the concatenation of everything it returns is
+ * bit-identical to b200gate_run on the concatenated input.  Output chunk i (samples [i cs, (i + 1) cs)) reads only input
+ * [i cs - pad, (i + 1) cs + pad), zero outside [0, N) (base.py:130-156); a recording of N <= cs samples is one padded
+ * chunk (base.py:222), which is only known at the end.  So after R samples have been received, exactly
+ *     E(R) = cs * max(0, floor((R - pad) / cs))  if R > cs,   E(R) = 0 otherwise
+ * have been returned: the latency is at most cs + pad - 1 samples.
+ *
+ * b200gate_stream_begin starts (or restarts) a stream of C channels of `dtype` on the handle.  The handle then keeps a
+ * device window of samples [max(0, E - pad), R) of every channel; its size depends on chunk_size, padding and C only,
+ * not on the stream length or the block sizes (a long push is consumed in slices of whole chunks).
+ * b200gate_stream_push appends samples [0, n) of each row of `in` (row stride in_stride) and writes the next *n_out
+ * samples of the result to out[c][0, *n_out).  in and out are host pointers, or device pointers with is_device = 1
+ * (then the call only enqueues on cuda_stream; *n_out is known at once).  Every push of a stream uses the same memory
+ * space; b200gate_stream_finish writes the rest of the result (< chunk_size + padding samples) into that space and
+ * closes the stream.  Errors: out_capacity < n + chunk_size (push) or < chunk_size + padding (finish): B200GATE_ERR_ARG
+ * before anything is written; a stationary gate without noise thresholds (b200gate_noise_stats /
+ * b200gate_set_noise_threshold, which may be called while the stream is open) when a chunk would be returned:
+ * B200GATE_ERR_STATE.  While a stream is open b200gate_run on the handle returns B200GATE_ERR_STATE.  After any other
+ * error the stream is closed. */
+int b200gate_stream_begin(b200gate_handle* h, int dtype, int64_t C);
+int b200gate_stream_push(b200gate_handle* h, const void* in, int64_t n, int64_t in_stride, int is_device,
+                         void* out, int64_t out_stride, int64_t out_capacity, int64_t* n_out, void* cuda_stream);
+int b200gate_stream_finish(b200gate_handle* h, void* out, int64_t out_stride, int64_t out_capacity,
+                           int64_t* n_out, void* cuda_stream);
 
 int b200gate_get_stats(const b200gate_handle* h, b200gate_stats* out);
 

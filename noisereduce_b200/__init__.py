@@ -7,6 +7,7 @@ The hot path (STFT -> noise threshold -> mask -> 2-D smoothing -> apply -> overl
 as hand-written sm_100a CUDA kernels in libb200gate.so (C ABI: include/b200gate.h).
 """
 from .noisereduce import reduce_noise
+from .spectralgate.stream import NoiseReduceStream
 
-__all__ = ["reduce_noise"]
+__all__ = ["reduce_noise", "NoiseReduceStream"]
 __version__ = "0.1.0"

@@ -16,6 +16,7 @@ _HERE = os.path.dirname(os.path.abspath(__file__))
 DEFAULT_LIB = os.path.join(_HERE, "libb200gate.so")
 
 ABI_VERSION = 1
+OK, ERR_ARG, ERR_CUDA, ERR_STATE, ERR_NOMEM = 0, -1, -2, -3, -4
 F32, I16, F64 = 0, 1, 2
 SURFACE_NUMPY, SURFACE_TORCH = 0, 1
 _DTYPES = {np.dtype(np.float32): F32, np.dtype(np.int16): I16, np.dtype(np.float64): F64}
@@ -29,6 +30,7 @@ EXPORTS = [
     "b200gate_debug_read_bits", "b200gate_debug_read_mask", "b200gate_debug_read_spec",
     "b200gate_run_sharded", "b200gate_peer_push", "b200gate_peer_barrier", "b200gate_torch_apply_masks",
     "b200gate_host_alloc", "b200gate_host_free",
+    "b200gate_stream_begin", "b200gate_stream_push", "b200gate_stream_finish",
 ]
 
 
@@ -110,6 +112,9 @@ class GateLibrary:
         d.b200gate_host_alloc.restype = vp
         d.b200gate_host_free.argtypes = [vp]
         d.b200gate_host_free.restype = None
+        d.b200gate_stream_begin.argtypes = [vp, C.c_int, i64]
+        d.b200gate_stream_push.argtypes = [vp, vp, i64, i64, C.c_int, vp, i64, i64, C.POINTER(i64), vp]
+        d.b200gate_stream_finish.argtypes = [vp, vp, i64, i64, C.POINTER(i64), vp]
 
 
 def peer_push(lib, src_ptr, peer_ptrs, rows, row_bytes, src_stride_bytes, dst_stride_bytes, n_ctas, stream):
@@ -297,6 +302,21 @@ class Gate:
     def torch_apply_masks_device(self, in_ptr, out_ptr, dtype, C_, N, in_stride, out_stride, stream=None):
         self._check(self.lib.dll.b200gate_torch_apply_masks(
             self._h, in_ptr, out_ptr, dtype_code(dtype), C_, N, in_stride, out_stride, 1, stream))
+
+    # -- streaming (b200gate_stream_*): pointers and sizes as in the header; the push / finish return n_out --------------
+    def stream_begin(self, dtype, C_):
+        self._check(self.lib.dll.b200gate_stream_begin(self._h, dtype_code(dtype), C_))
+
+    def stream_push(self, in_ptr, n, in_stride, is_device, out_ptr, out_stride, out_capacity, stream=None) -> int:
+        n_out = C.c_int64()
+        self._check(self.lib.dll.b200gate_stream_push(self._h, in_ptr, n, in_stride, 1 if is_device else 0, out_ptr,
+                                                      out_stride, out_capacity, C.byref(n_out), stream))
+        return n_out.value
+
+    def stream_finish(self, out_ptr, out_stride, out_capacity, stream=None) -> int:
+        n_out = C.c_int64()
+        self._check(self.lib.dll.b200gate_stream_finish(self._h, out_ptr, out_stride, out_capacity, C.byref(n_out), stream))
+        return n_out.value
 
     def set_range(self, mode: int, a: int = 0, b: int = 0):
         self._check(self.lib.dll.b200gate_set_range(self._h, mode, a, b))

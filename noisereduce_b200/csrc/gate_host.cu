@@ -101,6 +101,13 @@ struct b200gate_handle {
     void* d_slab_out[2] = {nullptr, nullptr};
     size_t slab_in_bytes[2] = {0, 0}, slab_out_bytes[2] = {0, 0};
     b200gate_stats stats{};
+    // streaming (b200gate_stream_*): a device window holding samples [s_lo, s_R) of every channel, row pitch s_cap
+    bool s_open = false;
+    int s_dtype = 0, s_is_device = -1;             // is_device of the stream's pushes (-1: none yet)
+    long long s_C = 0, s_R = 0, s_E = 0, s_lo = 0; // samples received / returned; first sample in the window
+    long long s_cap = 0, s_slice = 0, s_ocap = 0;  // window pitch, samples one slice appends at most, output pitch
+    void *d_swin = nullptr, *d_sout = nullptr;
+    size_t swin_bytes = 0, sout_bytes = 0;
     // debug taps
     long long dbg_chunk = -1, dbg_channel = -1;
     long long dbg_T = 0;
@@ -955,6 +962,8 @@ void b200gate_destroy(b200gate_handle* h) {
     g_device_pool.give(h->d_in, h->in_bytes, h->device);
     g_device_pool.give(h->d_out, h->out_bytes, h->device);
     g_device_pool.give(h->d_raw, h->raw_bytes, h->device);
+    g_device_pool.give(h->d_swin, h->swin_bytes, h->device);
+    g_device_pool.give(h->d_sout, h->sout_bytes, h->device);
     void* ptrs[] = {h->d_wa, h->d_ws, h->d_invn, h->d_thr4, h->d_gco, h->d_floor4, h->d_ef, h->d_tw, h->d_thr2_64,
                     h->d_wa64, h->d_cs64, h->d_tthr, h->d_wa2, h->d_ws2, h->d_w2k, h->d_invn2, h->d_cnt, h->d_dbg_spec,
                     h->d_dbg_mask, h->d_dbg_bits, h->d_gwa, h->d_gws, h->d_gw2, h->d_gthr, h->d_gcs, h->d_gtthr, h->d_gchirp, h->d_gbbr};
@@ -1211,15 +1220,17 @@ int b200gate_torch_set_noise(b200gate_handle* h, const void* xn, int dtype, int6
     return B200GATE_OK;
 }
 
-int b200gate_run(b200gate_handle* h, const void* in, void* out, int dtype, int64_t C, int64_t N, int64_t in_stride,
-                 int64_t out_stride, int is_device, void* stream) {
+// b200gate_run on input rows that hold only samples [in_first, N) (a stream's window, addressed through the virtual base
+// `in` = window - in_first): the row stride then only has to cover that span.
+static int run_core(b200gate_handle* h, const void* in, void* out, int dtype, int64_t C, int64_t N, int64_t in_stride,
+                    int64_t out_stride, int is_device, void* stream, int64_t in_first) {
     if (!h || !in || !out || C <= 0 || N <= 0 || dtype_size(dtype) == 0) return fail(h, B200GATE_ERR_ARG, "bad argument");
     const bool torch_sem = h->p.surface == B200GATE_SURFACE_TORCH;
     // torch.istft(center=True) length: n_fft + hop (T - 1) minus n_fft/2 at both ends (torchgate.py:255-262)
     const int64_t No = torch_sem ? (N / h->p.hop_length) * h->p.hop_length + (h->p.n_fft & 1) : N;
     // In a range mode only samples [o_lo, o_hi) of a row are addressed, so `out` may be a virtual base
     // (slab - o_lo) over rows as short as the range: the stride check below uses the range length.
-    if (in_stride < N || (out_stride < No && (torch_sem || h->range_mode == 0)))
+    if (in_stride < N - in_first || (out_stride < No && (torch_sem || h->range_mode == 0)))
         return fail(h, B200GATE_ERR_ARG, "row strides too small");
     if (torch_sem && N < 2 * h->p.win_length) return fail(h, B200GATE_ERR_ARG, "x must be bigger than %d", 2 * h->p.win_length);
     if (torch_sem && h->tthr_units > 1 && h->tthr_units != C)
@@ -2093,6 +2104,182 @@ int b200gate_run(b200gate_handle* h, const void* in, void* out, int dtype, int64
         if (rc) return rc;
     }
     h->stats.last_h2d_ms = h2d_ms;
+    return B200GATE_OK;
+}
+
+int b200gate_run(b200gate_handle* h, const void* in, void* out, int dtype, int64_t C, int64_t N, int64_t in_stride,
+                 int64_t out_stride, int is_device, void* stream) {
+    if (h && h->s_open) return fail(h, B200GATE_ERR_STATE, "a stream is open on this handle (b200gate_stream_finish first)");
+    return run_core(h, in, out, dtype, C, N, in_stride, out_stride, is_device, stream, 0);
+}
+
+// ---- streaming: the recording arrives in blocks (include/b200gate.h) --------------------------------------------------
+namespace {
+
+// samples returned once R have been received: every chunk whose padded span [i cs - pad, (i + 1) cs + pad) has arrived,
+// and nothing while the recording could still turn out to be one padded chunk (N <= chunk_size, base.py:222)
+long long stream_emitted(const b200gate_params& p, long long R) {
+    const long long cs = p.chunk_size;
+    return R > cs ? cs * std::max(0LL, (R - p.padding) / cs) : 0;
+}
+
+// A pinned staging buffer of at least `bytes` (host pushes of pageable memory), from the process-wide pool.
+int stream_pinned(b200gate_handle* h, void** buf, size_t* have, size_t bytes) {
+    if (*have >= bytes) return B200GATE_OK;
+    g_pinned_pool.give(*buf, *have);
+    *buf = g_pinned_pool.take(bytes, have);
+    if (!*buf) { *have = 0; return fail(h, B200GATE_ERR_NOMEM, "pinned staging buffer (%zu bytes)", bytes); }
+    return B200GATE_OK;
+}
+
+// Run chunks [E / cs, E_new / cs) (or, last == true, everything from E to the end of a recording of R samples) from the
+// window, write them to out + (E - first_col) columns, and advance E.  One run_core call: the batching of an offline run.
+int stream_emit(b200gate_handle* h, long long E_new, bool last, void* out, long long out_stride, long long first_col,
+                int is_device, cudaStream_t st) {
+    const b200gate_params& p = h->p;
+    const long long R = h->s_R, E = h->s_E, C = h->s_C;
+    const size_t es = dtype_size(h->s_dtype);
+    if (E_new <= E) return B200GATE_OK;
+    const bool stage = !is_device && !host_pointer_is_pinned(out);
+    int rc;
+    if (!is_device && (rc = ensure(h, &h->d_sout, &h->sout_bytes, (size_t)C * h->s_ocap * es))) return rc;
+    if (stage && (rc = stream_pinned(h, &h->hp_out[0], &h->hp_out_bytes[0], (size_t)C * h->s_ocap * es))) return rc;
+    const void* xv = (const char*)h->d_swin - (size_t)h->s_lo * es;
+    // host callers: the library's output buffer (pitch s_ocap, column 0 = sample E), then one copy out
+    void* yv = is_device ? (char*)out - (size_t)first_col * es : (char*)h->d_sout - (size_t)E * es;
+    const long long ys = is_device ? out_stride : h->s_ocap;
+    const int32_t mode0 = h->range_mode;
+    const long long a0 = h->range_a, b0 = h->range_b;
+    if (last && R <= p.chunk_size) h->range_mode = 0;          // one padded chunk: the whole recording
+    else { h->range_mode = 1; h->range_a = E / p.chunk_size; h->range_b = (E_new - 1) / p.chunk_size; }
+    rc = run_core(h, xv, yv, h->s_dtype, C, R, h->s_cap, ys, 1, st, h->s_lo);
+    h->range_mode = mode0; h->range_a = a0; h->range_b = b0;
+    if (rc) return rc;
+    if (!is_device) {
+        const long long m = E_new - E;
+        void* dst = (char*)out + (size_t)(E - first_col) * es;
+        CK(h, cudaMemcpy2DAsync(stage ? h->hp_out[0] : dst, stage ? (size_t)m * es : (size_t)out_stride * es, h->d_sout,
+                                (size_t)h->s_ocap * es, (size_t)m * es, (size_t)C, cudaMemcpyDeviceToHost, st));
+        CK(h, cudaStreamSynchronize(st));
+        if (stage) parallel_rows_copy(dst, (size_t)out_stride * es, h->hp_out[0], (size_t)m * es, (size_t)m * es, (size_t)C,
+                                      h->host_threads);
+    }
+    h->s_E = E_new;
+    return B200GATE_OK;
+}
+
+int stream_check_space(b200gate_handle* h, int is_device) {
+    if (!h->s_open) return fail(h, B200GATE_ERR_STATE, "no open stream (b200gate_stream_begin first)");
+    if (h->s_is_device >= 0 && h->s_is_device != (is_device ? 1 : 0))
+        return fail(h, B200GATE_ERR_ARG, "every push of a stream must use the same memory space (is_device)");
+    return B200GATE_OK;
+}
+
+}  // namespace
+
+int b200gate_stream_begin(b200gate_handle* h, int dtype, int64_t C) {
+    if (!h) return B200GATE_ERR_ARG;
+    h->s_open = false;
+    if (h->p.surface != B200GATE_SURFACE_NUMPY) return fail(h, B200GATE_ERR_ARG, "streaming needs the numpy surface");
+    if (h->p.chunk_size <= 0)
+        return fail(h, B200GATE_ERR_ARG, "streaming needs chunk_size > 0 (without chunks nothing can be returned early)");
+    const size_t es = dtype_size(dtype);
+    if (es == 0 || C <= 0) return fail(h, B200GATE_ERR_ARG, "bad argument");
+    const long long cs = h->p.chunk_size, pad = h->p.padding;
+    // window alignment: its first sample sits at an absolute index whose byte offset is a multiple of 16, and so does
+    // its row pitch, so the kernels see the addresses of an offline run of an aligned recording
+    const long long A = 16 / (long long)es;
+    // a push is consumed in slices of whole chunks, ~256 MB of input each (the slab size of the offline host path)
+    long long per = 256LL << 20;
+    if (const char* e = getenv("B200GATE_SLAB_MB")) per = std::max(1LL, atoll(e)) << 20;
+    long long k = std::max(1LL, std::min(64LL, per / std::max(1LL, C * cs * (long long)es)));
+    if (const char* e = getenv("B200GATE_STREAM_SLICE_CHUNKS")) k = std::max(1LL, atoll(e));   // tests / tuning
+    const long long S = k * cs;
+    // retained before a slice: [align(E - pad), R) with R - E < cs + pad, i.e. fewer than Lmax samples.  With a pitch of
+    // S + 2 Lmax the window is compacted only when the move's source and destination do not overlap.
+    const long long Lmax = 2 * pad + cs + A;
+    h->s_slice = S;
+    h->s_cap = (S + 2 * Lmax + A - 1) / A * A;
+    h->s_ocap = (S + cs + pad + A - 1) / A * A;                // a slice returns < S + cs samples, the end < cs + pad
+    int rc;
+    if ((rc = ensure(h, &h->d_swin, &h->swin_bytes, (size_t)C * h->s_cap * es))) return rc;
+    h->s_dtype = dtype; h->s_C = C; h->s_R = 0; h->s_E = 0; h->s_lo = 0; h->s_is_device = -1;
+    h->s_open = true;
+    return B200GATE_OK;
+}
+
+int b200gate_stream_push(b200gate_handle* h, const void* in, int64_t n, int64_t in_stride, int is_device, void* out,
+                         int64_t out_stride, int64_t out_capacity, int64_t* n_out, void* stream) {
+    if (!h) return B200GATE_ERR_ARG;
+    int rc;
+    if ((rc = stream_check_space(h, is_device))) return rc;
+    const b200gate_params& p = h->p;
+    const long long C = h->s_C;
+    if (!n_out || n < 0 || (n > 0 && (!in || in_stride < n)) || !out || out_stride < out_capacity)
+        return fail(h, B200GATE_ERR_ARG, "bad argument");
+    if (out_capacity < n + p.chunk_size)
+        return fail(h, B200GATE_ERR_ARG, "out_capacity %lld < n + chunk_size = %lld", (long long)out_capacity,
+                    (long long)(n + p.chunk_size));
+    const long long E0 = h->s_E, E_end = stream_emitted(p, h->s_R + n);
+    if (E_end > E0 && p.stationary && !h->have_thresh)
+        return fail(h, B200GATE_ERR_STATE, "stationary stream: set the noise thresholds before the first chunk is returned");
+    *n_out = E_end - E0;
+    if (n == 0) return B200GATE_OK;
+    h->s_is_device = is_device ? 1 : 0;
+    cudaStream_t st = (cudaStream_t)stream;
+    const size_t es = dtype_size(h->s_dtype);
+    const long long S = h->s_slice, A = 16 / (long long)es;
+    const bool stage_in = !is_device && !host_pointer_is_pinned(in);
+    if (stage_in && (rc = stream_pinned(h, &h->hp_in[0], &h->hp_in_bytes[0], (size_t)C * S * es))) return rc;
+    for (long long off = 0; off < n;) {
+        const long long s = std::min(S, n - off);
+        if (h->s_R - h->s_lo + s > h->s_cap) {                 // compact: keep [align(E - pad), R)
+            const long long lo = std::max(0LL, h->s_E - p.padding) / A * A, L = h->s_R - lo;
+            if (L > 0)
+                CK(h, cudaMemcpy2DAsync(h->d_swin, (size_t)h->s_cap * es, (char*)h->d_swin + (size_t)(lo - h->s_lo) * es,
+                                        (size_t)h->s_cap * es, (size_t)L * es, (size_t)C, cudaMemcpyDeviceToDevice, st));
+            h->s_lo = lo;
+        }
+        // the slice's samples cross to the device once, behind the retained ones
+        void* dst = (char*)h->d_swin + (size_t)(h->s_R - h->s_lo) * es;
+        const void* src = (const char*)in + (size_t)off * es;
+        size_t spitch = (size_t)in_stride * es;
+        if (stage_in) {
+            CK(h, cudaStreamSynchronize(st));                   // the previous slice has left the staging buffer
+            parallel_rows_copy(h->hp_in[0], (size_t)s * es, src, spitch, (size_t)s * es, (size_t)C, h->host_threads);
+            src = h->hp_in[0];
+            spitch = (size_t)s * es;
+        }
+        CK(h, cudaMemcpy2DAsync(dst, (size_t)h->s_cap * es, src, spitch, (size_t)s * es, (size_t)C,
+                                is_device ? cudaMemcpyDeviceToDevice : cudaMemcpyHostToDevice, st));
+        h->s_R += s;
+        off += s;
+        if ((rc = stream_emit(h, stream_emitted(p, h->s_R), false, out, out_stride, E0, is_device, st))) {
+            h->s_open = false;
+            return rc;
+        }
+    }
+    if (!is_device) CK(h, cudaStreamSynchronize(st));
+    return B200GATE_OK;
+}
+
+int b200gate_stream_finish(b200gate_handle* h, void* out, int64_t out_stride, int64_t out_capacity, int64_t* n_out,
+                           void* stream) {
+    if (!h) return B200GATE_ERR_ARG;
+    int rc;
+    if ((rc = stream_check_space(h, h->s_is_device > 0))) return rc;
+    const b200gate_params& p = h->p;
+    if (!n_out || !out || out_stride < out_capacity) return fail(h, B200GATE_ERR_ARG, "bad argument");
+    if (out_capacity < p.chunk_size + p.padding)
+        return fail(h, B200GATE_ERR_ARG, "out_capacity %lld < chunk_size + padding = %lld", (long long)out_capacity,
+                    (long long)(p.chunk_size + p.padding));
+    const long long E0 = h->s_E, R = h->s_R;
+    if (R > E0 && p.stationary && !h->have_thresh)
+        return fail(h, B200GATE_ERR_STATE, "stationary stream: set the noise thresholds before the first chunk is returned");
+    rc = stream_emit(h, R, true, out, out_stride, E0, h->s_is_device > 0, (cudaStream_t)stream);
+    h->s_open = false;
+    if (rc) return rc;
+    *n_out = R - E0;
     return B200GATE_OK;
 }
 

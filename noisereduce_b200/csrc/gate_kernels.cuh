@@ -403,8 +403,11 @@ __global__ void __launch_bounds__(kThreads, B200_K1_MINBLOCKS) k1_analyze(const 
         xrow = static_cast<const T*>(a.x) + (long long)c * g.in_stride;
     };
     // Request the window of pair (tt, tt + 1) of a unit into this warp's buffer when it lies inside the chunk and the
-    // recording and the 16-byte-aligned span covering it lies inside the row.  Returns the window's element offset in
-    // the buffer, or -1: the pair is then loaded directly.  Warp-uniform; every lane has finished reading the buffer.
+    // recording and the 16-byte-aligned span covering it lies inside the samples the chunk reads,
+    // [max(0, i1), min(n_total, i1 + Lp)).  (Bounding it by the row instead let the aligned span reach past the rows a
+    // caller staged or streamed -- [w_lo, w_hi) of b200gate_run -- by up to 15 bytes at either end.)  Returns the
+    // window's element offset in the buffer, or -1: the pair is then loaded directly.  Warp-uniform; every lane has
+    // finished reading the buffer.
     auto request = [&](const T* xr_, long long i1_, int tt) -> int {
         if (!kBulk) return -1;
         const long long bb = (long long)tt * H - kN / 2;
@@ -412,7 +415,8 @@ __global__ void __launch_bounds__(kThreads, B200_K1_MINBLOCKS) k1_analyze(const 
         const unsigned long long src = reinterpret_cast<unsigned long long>(xr_ + i1_ + bb);
         const unsigned long long lo = src & ~15ull;
         const unsigned long long hi = (src + 32 * (32 + HR) * sizeof(T) + 15) & ~15ull;
-        if (lo < reinterpret_cast<unsigned long long>(xr_) || hi > reinterpret_cast<unsigned long long>(xr_ + g.n_total))
+        const long long r_lo = i1_ > 0 ? i1_ : 0, r_hi = i1_ + g.Lp < g.n_total ? i1_ + g.Lp : g.n_total;
+        if (lo < reinterpret_cast<unsigned long long>(xr_ + r_lo) || hi > reinterpret_cast<unsigned long long>(xr_ + r_hi))
             return -1;
         fence_proxy_async_smem();
         __syncwarp();

@@ -1,4 +1,5 @@
 from .nonstationary import SpectralGateNonStationary
 from .stationary import SpectralGateStationary
+from .stream import NoiseReduceStream
 
-__all__ = ["SpectralGateStationary", "SpectralGateNonStationary"]
+__all__ = ["SpectralGateStationary", "SpectralGateNonStationary", "NoiseReduceStream"]

@@ -21,6 +21,14 @@ def _smoothing_filter(n_grad_freq, n_grad_time):
     return filt / np.sum(filt)
 
 
+def samples_for_device(y2d):
+    """float32 / int16 / float64 go to the library as they are; any other dtype takes the
+    reference's own route -- promoted to float64 (base.py:140) -- and is cast back on return."""
+    if y2d.dtype in (np.float32, np.int16, np.float64):
+        return np.ascontiguousarray(y2d)
+    return np.ascontiguousarray(y2d, dtype=np.float64)
+
+
 class SpectralGate:
     def __init__(
         self,
@@ -123,11 +131,7 @@ class SpectralGate:
         )
 
     def _samples_for_device(self, y2d):
-        """float32 / int16 / float64 go to the library as they are; any other dtype takes the
-        reference's own route -- promoted to float64 (base.py:140) -- and is cast back on return."""
-        if y2d.dtype in (np.float32, np.int16, np.float64):
-            return np.ascontiguousarray(y2d)
-        return np.ascontiguousarray(y2d, dtype=np.float64)
+        return samples_for_device(y2d)
 
     def _run(self, y2d, lo=0, hi=None):
         """One library call; returns columns [lo, hi) of the (partially written) output rows."""

@@ -2,7 +2,7 @@
 import numpy as np
 
 from .. import _cabi
-from .base import SpectralGate
+from .base import SpectralGate, samples_for_device
 
 
 class SpectralGateStationary(SpectralGate):
@@ -51,38 +51,8 @@ class SpectralGateStationary(SpectralGate):
                       clip_noise=1 if clip_noise_stationary else 0)
         self._params = params
         self._gate = _cabi.Gate(**params)
-        # stationary.py:61-81 on the device: channel mean in the input dtype, clip, STFT, dB with the
-        # 80 dB floor, per-bin mean / std over time, threshold
-        clip = noise
-        if noise.dtype not in (np.float32, np.int16, np.float64):
-            # the reference collapses the clip with np.mean in the clip's own dtype rules (stationary.py:61): float16 stays
-            # float16 (float32 accumulation, rounded), integers / bool become float64 -- numpy decides, the device gets the result
-            clip = np.mean(noise, axis=0)[None, :]
-            if clip.dtype not in (np.float32, np.float64):
-                clip = clip.astype(np.float32)
-        n_eff = clip.shape[1]
-        if clip_noise_stationary and self._chunk_size is not None:
-            n_eff = min(n_eff, int(self._chunk_size))                         # stationary.py:63-64
-        noverlap = self._win_length - self._hop_length
-        if n_eff < self._win_length:
-            # scipy.signal.stft on a clip shorter than the window shrinks the window to the clip (nperseg = len(x), with a
-            # warning) and then insists on noverlap < nperseg; the reference inherits both behaviours (stationary.py:67-73)
-            if noverlap >= n_eff:
-                raise ValueError("noverlap must be less than nperseg.")
-            short = dict(params)
-            short.update(win_length=int(n_eff), hop_length=int(n_eff - noverlap))
-            stats_gate = _cabi.Gate(**short)
-            try:
-                stats_gate.noise_stats_host(self._samples_for_device(clip[:, :n_eff]))
-                self.mean_freq_noise, self.std_freq_noise = stats_gate.noise_mean_std()
-                self.noise_thresh = stats_gate.noise_threshold()
-            finally:
-                stats_gate.close()
-            self._gate.set_noise_threshold(self.noise_thresh)
-        else:
-            self._gate.noise_stats_host(self._samples_for_device(clip))
-            self.mean_freq_noise, self.std_freq_noise = self._gate.noise_mean_std()
-            self.noise_thresh = self._gate.noise_threshold()
+        self.mean_freq_noise, self.std_freq_noise, self.noise_thresh = install_noise_thresholds(
+            self._gate, params, noise, self._chunk_size if clip_noise_stationary else None)
 
     def _unit_gate_params(self):
         p = dict(self._params)
@@ -98,3 +68,42 @@ class SpectralGateStationary(SpectralGate):
         the input dtype, clipped to chunk_size.  Computed on demand -- the thresholds come from the device."""
         n = self._noise2d[:, : self._chunk_size] if self._clip_noise else self._noise2d
         return np.mean(n, axis=0)
+
+
+def install_noise_thresholds(gate, params, noise, clip_to):
+    """stationary.py:61-81 on the device: channel mean in the input dtype, clip to `clip_to` samples (chunk_size when
+    clip_noise_stationary, else None), STFT, dB with the 80 dB floor, per-bin mean / std over time, threshold.  `noise`
+    is [C, n]; `gate` is a stationary handle created from `params`, which receives the thresholds.  Returns
+    (mean, std, threshold) per bin."""
+    clip = noise
+    if noise.dtype not in (np.float32, np.int16, np.float64):
+        # the reference collapses the clip with np.mean in the clip's own dtype rules (stationary.py:61): float16 stays
+        # float16 (float32 accumulation, rounded), integers / bool become float64 -- numpy decides, the device gets the result
+        clip = np.mean(noise, axis=0)[None, :]
+        if clip.dtype not in (np.float32, np.float64):
+            clip = clip.astype(np.float32)
+    n_eff = clip.shape[1]
+    if clip_to is not None:
+        n_eff = min(n_eff, int(clip_to))                                      # stationary.py:63-64
+    win_length, hop_length = params["win_length"], params["hop_length"]
+    noverlap = win_length - hop_length
+    if n_eff < win_length:
+        # scipy.signal.stft on a clip shorter than the window shrinks the window to the clip (nperseg = len(x), with a
+        # warning) and then insists on noverlap < nperseg; the reference inherits both behaviours (stationary.py:67-73)
+        if noverlap >= n_eff:
+            raise ValueError("noverlap must be less than nperseg.")
+        short = dict(params)
+        short.update(win_length=int(n_eff), hop_length=int(n_eff - noverlap))
+        stats_gate = _cabi.Gate(lib=gate.lib, **short)
+        try:
+            stats_gate.noise_stats_host(samples_for_device(clip[:, :n_eff]))
+            mean, std = stats_gate.noise_mean_std()
+            thresh = stats_gate.noise_threshold()
+        finally:
+            stats_gate.close()
+        gate.set_noise_threshold(thresh)
+    else:
+        gate.noise_stats_host(samples_for_device(clip))
+        mean, std = gate.noise_mean_std()
+        thresh = gate.noise_threshold()
+    return mean, std, thresh
