@@ -44,6 +44,10 @@ enum {
 };
 
 enum { B200GATE_F32 = 0, B200GATE_I16 = 1, B200GATE_F64 = 2 };     /* sample dtypes */
+/* further sample formats, taken by b200gate_convert only (the gate itself runs F32 / I16 / F64); BOOL is one byte 0/1 */
+enum { B200GATE_BOOL = 3, B200GATE_I8 = 4, B200GATE_U8 = 5, B200GATE_U16 = 6, B200GATE_I32 = 7, B200GATE_U32 = 8,
+       B200GATE_I64 = 9, B200GATE_U64 = 10, B200GATE_F16 = 11 };
+enum { B200GATE_CONVERT_CAST = 0, B200GATE_CONVERT_CHANNEL_MEAN = 1 };   /* b200gate_convert operations */
 enum { B200GATE_SURFACE_NUMPY = 0, B200GATE_SURFACE_TORCH = 1 };   /* which reference semantics */
 
 /* Resolved operator parameters.  The Python shims resolve defaults exactly as the reference does
@@ -196,6 +200,26 @@ int b200gate_stream_finish(b200gate_handle* h, void* out, int64_t out_stride, in
                            int64_t* n_out, void* cuda_stream);
 
 int b200gate_get_stats(const b200gate_handle* h, b200gate_stats* out);
+
+/* ---- sample formats of device-resident callers ----------------------------------------------------------------------
+ * The reference runs any dtype other than float32 / int16 / float64 through float64 (base.py:140) and casts the result
+ * back with ndarray.astype (base.py:218-226); its stationary thresholds start from np.mean(noise, axis=0) in the clip's
+ * own dtype rules (stationary.py:61).  For samples already on the device these steps are kernels, bit-identical to
+ * numpy on x86-64 (noisereduce_b200/csrc/gate_convert.cuh has the rules):
+ *   B200GATE_CONVERT_CAST: dst[c][j] = src[c][j] for c < C, j < N, converted; one of src_dtype / dst_dtype is
+ *     B200GATE_F64.  To float64 the cast is exact except for 64-bit integers beyond 2^53 (round to nearest even); from
+ *     float64 it is ndarray.astype on unit-stride rows: float16 rounds once, bool is v != 0, integers truncate, and
+ *     NaN, +-inf and out-of-range values map as x86-64's cvttsd2si does.
+ *   B200GATE_CONVERT_CHANNEL_MEAN: dst[j] = mean over c of src[c][j], j < N, as float64 (dst_dtype B200GATE_F64,
+ *     dst_stride ignored): float16 / float32 sum in float32 in channel order and float16 rounds the mean to half; every
+ *     other format sums in float64 in channel order.  (numpy sums pairwise over a contiguous axis: for channel-adjacent
+ *     layouts this equals np.mean of the row-major copy.)
+ * src / dst are device pointers (may be NULL when there is nothing to convert) with row strides in elements (>= N
+ * when C > 1).  No handle: the work is enqueued on
+ * cuda_stream on the current device, and the call returns without waiting.  Errors are read with
+ * b200gate_last_error(NULL). */
+int b200gate_convert(int op, const void* src, int src_dtype, int64_t src_stride, void* dst, int dst_dtype,
+                     int64_t dst_stride, int64_t C, int64_t N, void* cuda_stream);
 
 /* Page-locked host buffers from the library's process-wide pool (the same pool the slab pipeline stages pageable
  * caller memory through).  A result array the reference would np.empty() (base.py:181-187 uses a temp-file memmap)

@@ -20,6 +20,12 @@ OK, ERR_ARG, ERR_CUDA, ERR_STATE, ERR_NOMEM = 0, -1, -2, -3, -4
 F32, I16, F64 = 0, 1, 2
 SURFACE_NUMPY, SURFACE_TORCH = 0, 1
 _DTYPES = {np.dtype(np.float32): F32, np.dtype(np.int16): I16, np.dtype(np.float64): F64}
+# b200gate_convert's further formats (include/b200gate.h)
+BOOL, I8, U8, U16, I32, U32, I64, U64, F16 = 3, 4, 5, 6, 7, 8, 9, 10, 11
+CONVERT_CAST, CONVERT_CHANNEL_MEAN = 0, 1
+_FORMATS = {**_DTYPES, **{np.dtype(t): c for t, c in (
+    (np.bool_, BOOL), (np.int8, I8), (np.uint8, U8), (np.uint16, U16), (np.int32, I32), (np.uint32, U32),
+    (np.int64, I64), (np.uint64, U64), (np.float16, F16))}}
 
 EXPORTS = [
     "b200gate_create", "b200gate_destroy", "b200gate_last_error", "b200gate_noise_stats",
@@ -30,7 +36,7 @@ EXPORTS = [
     "b200gate_debug_read_bits", "b200gate_debug_read_mask", "b200gate_debug_read_spec",
     "b200gate_run_sharded", "b200gate_peer_push", "b200gate_peer_barrier", "b200gate_torch_apply_masks",
     "b200gate_host_alloc", "b200gate_host_free",
-    "b200gate_stream_begin", "b200gate_stream_push", "b200gate_stream_finish",
+    "b200gate_stream_begin", "b200gate_stream_push", "b200gate_stream_finish", "b200gate_convert",
 ]
 
 
@@ -69,7 +75,12 @@ class GateError(RuntimeError):
 
 
 class GateLibrary:
-    """A loaded libb200gate with typed prototypes."""
+    """A loaded libb200gate with typed prototypes.
+
+    ``simulated_device`` (tests only, default False): the library is the CPU simulator build, whose "device" pointers
+    are host pointers, and CPU torch tensors take the CUDA-tensor route of reduce_noise() / NoiseReduceStream."""
+
+    simulated_device = False
 
     def __init__(self, path: str = DEFAULT_LIB):
         if not os.path.exists(path):
@@ -115,6 +126,23 @@ class GateLibrary:
         d.b200gate_stream_begin.argtypes = [vp, C.c_int, i64]
         d.b200gate_stream_push.argtypes = [vp, vp, i64, i64, C.c_int, vp, i64, i64, C.POINTER(i64), vp]
         d.b200gate_stream_finish.argtypes = [vp, vp, i64, i64, C.POINTER(i64), vp]
+        d.b200gate_convert.argtypes = [C.c_int, vp, C.c_int, i64, vp, C.c_int, i64, i64, i64, vp]
+
+
+def format_code(dt) -> int:
+    """b200gate_convert's code for a numpy dtype (every real dtype numpy and torch share)."""
+    dt = np.dtype(dt)
+    if dt not in _FORMATS:
+        raise TypeError(f"unsupported sample dtype {dt}")
+    return _FORMATS[dt]
+
+
+def convert(lib, op, src_ptr, src_dtype, src_stride, dst_ptr, dst_dtype, dst_stride, C_, N, stream=None):
+    """b200gate_convert on device pointers (include/b200gate.h): op CONVERT_CAST or CONVERT_CHANNEL_MEAN."""
+    rc = lib.dll.b200gate_convert(op, src_ptr, format_code(src_dtype), src_stride, dst_ptr, format_code(dst_dtype),
+                                  dst_stride, C_, N, stream)
+    if rc != 0:
+        raise GateError(rc, lib.dll.b200gate_last_error(None).decode())
 
 
 def peer_push(lib, src_ptr, peer_ptrs, rows, row_bytes, src_stride_bytes, dst_stride_bytes, n_ctas, stream):

@@ -11,6 +11,7 @@
 #include "gate_dual.cuh"
 #include "gate_peer.cuh"
 #include "gate_generic.cuh"
+#include "gate_convert.cuh"
 
 #include <math.h>
 #include <cmath>
@@ -1028,6 +1029,67 @@ int b200gate_set_window(b200gate_handle* h, const float* window, int32_t win_len
     if (win_length != h->p.n_fft) return fail(h, B200GATE_ERR_ARG, "window length %d != n_fft %d", win_length, h->p.n_fft);
     h->user_window.assign(window, window + win_length);
     return build_static_tables(h);
+}
+
+}  // extern "C"
+
+namespace {
+// run `stmt` with the constant D bound to the format code `dt` (any code cv_size knows)
+#define B200_WITH_FORMAT(dt, ...)                                                                          \
+    switch (dt) {                                                                                          \
+        case B200GATE_F32: { constexpr int D = B200GATE_F32; __VA_ARGS__; } break;                          \
+        case B200GATE_I16: { constexpr int D = B200GATE_I16; __VA_ARGS__; } break;                          \
+        case B200GATE_F64: { constexpr int D = B200GATE_F64; __VA_ARGS__; } break;                          \
+        case B200GATE_BOOL: { constexpr int D = B200GATE_BOOL; __VA_ARGS__; } break;                        \
+        case B200GATE_I8: { constexpr int D = B200GATE_I8; __VA_ARGS__; } break;                            \
+        case B200GATE_U8: { constexpr int D = B200GATE_U8; __VA_ARGS__; } break;                            \
+        case B200GATE_U16: { constexpr int D = B200GATE_U16; __VA_ARGS__; } break;                          \
+        case B200GATE_I32: { constexpr int D = B200GATE_I32; __VA_ARGS__; } break;                          \
+        case B200GATE_U32: { constexpr int D = B200GATE_U32; __VA_ARGS__; } break;                          \
+        case B200GATE_I64: { constexpr int D = B200GATE_I64; __VA_ARGS__; } break;                          \
+        case B200GATE_U64: { constexpr int D = B200GATE_U64; __VA_ARGS__; } break;                          \
+        default: { constexpr int D = B200GATE_F16; __VA_ARGS__; } break;                                   \
+    }
+
+// elementwise, bandwidth-bound: enough CTAs to fill the device, each striding over a row's columns
+dim3 convert_grid(long long C, long long N) {
+    const int gy = (int)std::min<long long>(C, 1024);
+    return dim3(grid_1d(N, 256, std::max(1, 4096 / gy)), gy);
+}
+}  // namespace
+
+extern "C" {
+
+int b200gate_convert(int op, const void* src, int src_dtype, int64_t src_stride, void* dst, int dst_dtype,
+                     int64_t dst_stride, int64_t C, int64_t N, void* stream) {
+    if (((!src || !dst) && C > 0 && N > 0) || C < 0 || N < 0 || cv_size(src_dtype) == 0 || cv_size(dst_dtype) == 0 ||
+        (C > 1 && src_stride < N))
+        return fail(nullptr, B200GATE_ERR_ARG, "b200gate_convert: bad argument");
+    cudaStream_t st = (cudaStream_t)stream;
+    if (op == B200GATE_CONVERT_CAST) {
+        if (src_dtype != B200GATE_F64 && dst_dtype != B200GATE_F64)
+            return fail(nullptr, B200GATE_ERR_ARG, "b200gate_convert: a cast goes to or from float64");
+        if (C > 1 && dst_stride < N) return fail(nullptr, B200GATE_ERR_ARG, "b200gate_convert: dst_stride < N");
+        if (C == 0 || N == 0) return B200GATE_OK;
+        const dim3 grid = convert_grid(C, N);
+        if (dst_dtype == B200GATE_F64) {
+            B200_WITH_FORMAT(src_dtype, { auto kern_ = k_convert<D, B200GATE_F64>;
+                B200_LAUNCH(kern_, grid, dim3(256), 0, st, src, (long long)src_stride, dst, (long long)dst_stride, (long long)C, (long long)N); });
+        } else {
+            B200_WITH_FORMAT(dst_dtype, { auto kern_ = k_convert<B200GATE_F64, D>;
+                B200_LAUNCH(kern_, grid, dim3(256), 0, st, src, (long long)src_stride, dst, (long long)dst_stride, (long long)C, (long long)N); });
+        }
+    } else if (op == B200GATE_CONVERT_CHANNEL_MEAN) {
+        if (dst_dtype != B200GATE_F64 || C == 0)
+            return fail(nullptr, B200GATE_ERR_ARG, "b200gate_convert: the channel mean takes C >= 1 and a float64 dst");
+        if (N == 0) return B200GATE_OK;
+        B200_WITH_FORMAT(src_dtype, { auto kern_ = k_channel_mean<D>;
+            B200_LAUNCH(kern_, dim3(grid_1d(N, 256, 4096)), dim3(256), 0, st, src, (long long)src_stride, (double*)dst, (long long)C, (long long)N); });
+    } else {
+        return fail(nullptr, B200GATE_ERR_ARG, "b200gate_convert: unknown operation %d", op);
+    }
+    CK(nullptr, cudaGetLastError());
+    return B200GATE_OK;
 }
 
 int b200gate_channel_sum(b200gate_handle* h, const void* y, int dtype, int64_t C, int64_t n, int64_t stride,

@@ -36,7 +36,8 @@ class SpectralGateNonStationary(SpectralGate):
                       thresh_n_mult=float(thresh_n_mult_nonstationary),
                       sigmoid_slope=float(sigmoid_slope_nonstationary))
         self._params = params
-        self._gate = _cabi.Gate(**params)
+        with self._on_device():
+            self._gate = _cabi.Gate(**params)
 
     def _unit_gate_params(self):
         p = dict(self._params)

@@ -7,10 +7,13 @@ zeros outside [0, N) (base.py:130-156), and the stationary thresholds come from 
 samples (stationary.py:47-81).  So a stream can return chunk i as soon as sample (i + 1) cs + pad has arrived, and what
 it returns, concatenated, is bit-identical to reduce_noise() on the concatenated input.
 """
+import contextlib
+import sys
+
 import numpy as np
 
 from .. import _cabi
-from .base import SpectralGate, samples_for_device
+from .base import KERNEL_DTYPES, DeviceSite, SpectralGate, is_device_tensor, numpy_dtype_of, samples_for_device
 from .stationary import install_noise_thresholds
 
 
@@ -36,6 +39,17 @@ class NoiseReduceStream:
     float32, int16 and float64 blocks go to the GPU as they are; any other real dtype is promoted to float64 per block
     and the result cast back, as reduce_noise() does.  The stationary gate without y_noise takes its thresholds from the
     first min(N, chunk_size) samples of the stream (clip_noise_stationary=True, reduce_noise()'s default).
+
+    Blocks may be torch CUDA tensors; push() and finish() then return CUDA tensors on the same device, with the same
+    bits.  Each push only enqueues work on the device's current torch stream (b200gate_stream_push with device pointers),
+    except the one that completes the stationary noise clip, which is collected on the device and whose statistics are
+    read back (the host waits for that stream).  Each returned tensor holds exactly its own samples; a push that returns
+    nothing returns an empty tensor without storage.  The first block fixes the memory space and the device: a later
+    block from the other memory space or another device raises ValueError.  y_noise may be a host array (its statistics
+    are computed as reduce_noise() does) or a CUDA tensor on the blocks' device.  Host waits for the whole device: the
+    handle's destruction (when the stream object is freed) synchronises the device before it releases its buffers, and
+    so does the one-time remaking of the handle on the first CUDA block's device when it was made on another device,
+    or before torch had initialised CUDA.
 
     The device holds a window of about 2 * padding + chunk_size samples per channel plus one slice of input, whatever
     the stream length or block sizes.  Not supported: chunk_size=None (the whole recording is one unit, so nothing could
@@ -73,21 +87,43 @@ class NoiseReduceStream:
         self.chunk_size, self.padding = int(chunk_size), int(padding)
         self._params = params
         self._clip_to = self.chunk_size if clip_noise_stationary else None
-        self._gate = _cabi.Gate(**params)
         self._dtype = None                  # of the first block
+        self._kdt = None                    # the dtype the gate runs: the first block's, or float64 (promoted)
+        self._site = None                   # CUDA-tensor blocks: their device (fixed by the first block)
         self._received = 0
         self._returned = 0
         self._closed = False
         self._clip = None                   # stationary without y_noise: the first chunk_size samples, [C, chunk_size]
         self._need_thresholds = False
-        if stationary:
-            if y_noise is None:
-                self._need_thresholds = True
-            else:                                                   # stationary.py:51-59
+        self._thresh = None                 # thresholds from y_noise, kept for a handle remade on the blocks' device
+        self._gate_device = None            # the CUDA device the handle was created on, where known
+        noise = None
+        if stationary and y_noise is None:
+            self._need_thresholds = True
+        elif stationary:                                            # stationary.py:51-59
+            if is_device_tensor(y_noise):
+                self._site = DeviceSite(y_noise)                    # the blocks must then be on y_noise's device
+                noise = y_noise
+            else:
                 noise = np.array(y_noise)
-                if noise.ndim == 1:
-                    noise = np.expand_dims(noise, 0)
-                install_noise_thresholds(self._gate, params, noise, self._clip_to)
+            noise = noise[None, :] if noise.ndim == 1 else noise
+        torch = sys.modules.get("torch")
+        if self._site is not None:
+            self._gate_device = self._site.device
+        elif torch is not None and torch.cuda.is_initialized():
+            self._gate_device = torch.device("cuda", torch.cuda.current_device())
+        # The handle is made here, so that the library's argument checks and y_noise's errors (a clip too short for
+        # the window) are raised by the constructor, as reduce_noise() raises them.
+        with self._on_device():
+            self._gate = _cabi.Gate(**params)
+            if noise is not None:
+                self._thresh = install_noise_thresholds(self._gate, params, noise, self._clip_to, self._stream())[2]
+
+    def _on_device(self):
+        return contextlib.nullcontext() if self._site is None else self._site.active()
+
+    def _stream(self):
+        return None if self._site is None else self._site.stream
 
     # -- emission rule --------------------------------------------------------------------------------------------
     def emitted(self, received=None):
@@ -108,27 +144,59 @@ class NoiseReduceStream:
     def _rows(self, block):
         if self._closed:
             raise ValueError("push() after finish(): the stream is closed")
-        x = np.asarray(block)
-        if np.iscomplexobj(x):
-            raise ValueError("Waveform must be real-valued")
+        on_device = is_device_tensor(block)
+        if self._dtype is not None and on_device != (self._site is not None):
+            raise ValueError("a stream's blocks stay in the memory space of its first block (CUDA tensors or host arrays)")
+        if on_device:
+            x, dt = block, numpy_dtype_of(block)
+            if self._site is not None:
+                self._site.check_same_device(x, "this block")
+        else:
+            x = np.asarray(block)
+            if np.iscomplexobj(x):
+                raise ValueError("Waveform must be real-valued")
+            dt = x.dtype
         if self.n_channels is None:
             if x.ndim != 1:
-                raise ValueError(f"this stream takes 1-D blocks (n_channels=None), got shape {x.shape}")
+                raise ValueError(f"this stream takes 1-D blocks (n_channels=None), got shape {tuple(x.shape)}")
             x = x[None, :]
         elif x.ndim != 2 or x.shape[0] != self.n_channels:
-            raise ValueError(f"expected a [{self.n_channels}, n] block, got shape {x.shape}")
+            raise ValueError(f"expected a [{self.n_channels}, n] block, got shape {tuple(x.shape)}")
         if self._dtype is None:
-            self._dtype = x.dtype
-            dev = samples_for_device(x[:, :0]).dtype
-            self._gate.stream_begin(dev, x.shape[0])
-        elif x.dtype != self._dtype:
-            raise ValueError(f"block dtype {x.dtype} differs from the stream's dtype {self._dtype}")
+            if on_device:
+                self._bind_device(x)
+            elif self._site is not None:
+                raise ValueError("y_noise is a CUDA tensor: the stream's blocks must be CUDA tensors on its device")
+            self._dtype = dt
+            self._kdt = dt if dt in KERNEL_DTYPES else np.dtype(np.float64)
+            with self._on_device():
+                self._gate.stream_begin(self._kdt, x.shape[0])
+        elif dt != self._dtype:
+            raise ValueError(f"block dtype {dt} differs from the stream's dtype {self._dtype}")
         return x
 
+    def _bind_device(self, x):
+        """The first block is a CUDA tensor: the stream runs on its device.  A handle made on another device, or on one
+        that is not known (torch had not initialised CUDA when the stream was constructed), is remade there once, with
+        y_noise's thresholds copied over rather than recomputed; closing the old handle waits for the device."""
+        if self._site is None:
+            self._site = DeviceSite(x)
+        if self._site.cuda and self._gate_device != self._site.device:
+            self._gate.close()
+            with self._site.active():
+                self._gate = _cabi.Gate(**self._params)
+                if self._thresh is not None:
+                    self._gate.set_noise_threshold(self._thresh)
+        self._gate_device = self._site.device
+
     def _collect_noise(self, x):
-        """Keep the first chunk_size samples; once they are all here, set the thresholds from them."""
+        """Keep the first chunk_size samples; once they are all here, set the thresholds from them.  CUDA-tensor blocks
+        are collected on their device."""
         if self._clip is None:
-            self._clip = np.empty((x.shape[0], self.chunk_size), dtype=x.dtype)
+            if self._site is None:
+                self._clip = np.empty((x.shape[0], self.chunk_size), dtype=x.dtype)
+            else:
+                self._clip = self._site.empty((x.shape[0], self.chunk_size), self._dtype)
         r0 = self._received
         take = min(x.shape[1], self.chunk_size - r0)
         if take > 0:
@@ -137,11 +205,21 @@ class NoiseReduceStream:
             self._set_stream_thresholds(self.chunk_size)
 
     def _set_stream_thresholds(self, n):
-        install_noise_thresholds(self._gate, self._params, self._clip[:, :n], self._clip_to)
+        install_noise_thresholds(self._gate, self._params, self._clip[:, :n], self._clip_to, self._stream())
         self._need_thresholds = False
         self._clip = None
 
     def _result(self, out, m):
+        if self._site is not None:
+            # Device memory is committed when allocated: a result holds its own m columns only, never the push's whole
+            # [C, n + chunk_size] output buffer (callers keep many results to concatenate them).
+            if m == 0:
+                out = self._site.empty((out.shape[0], 0), self._dtype)
+            elif self._kdt == self._dtype:
+                out = out[:, :m].clone(memory_format=self._site.torch.contiguous_format)
+            else:
+                out = self._site.cast_back(out[:, :m], self._dtype)     # (a new [C, m] tensor)
+            return out[0] if self.n_channels is None else out
         out = out[:, :m] if m > 0 else np.empty((out.shape[0], 0), out.dtype)    # (an empty result holds no buffer)
         if out.dtype != self._dtype:
             with np.errstate(invalid="ignore"):
@@ -150,8 +228,13 @@ class NoiseReduceStream:
 
     def push(self, block):
         """Append `block` ([n_channels, n], or [n] when n_channels is None) and return the next samples of the result
-        ([n_channels, m] / [m]); m = E(R + n) - E(R) is a multiple of chunk_size and may be 0."""
+        ([n_channels, m] / [m]); m = E(R + n) - E(R) is a multiple of chunk_size and may be 0.  A CUDA tensor block
+        returns a CUDA tensor; the call only enqueues work on the device's current torch stream, except when it
+        completes the stationary noise clip (the thresholds are read back once)."""
         x = self._rows(block)
+        if self._site is not None:
+            with self._site.active():
+                return self._push_device(x)
         if self._need_thresholds:
             self._collect_noise(x)
         C, n = x.shape
@@ -168,6 +251,22 @@ class NoiseReduceStream:
         self._returned += m
         return self._result(out, m)
 
+    def _push_device(self, x):
+        site = self._site
+        if self._need_thresholds:
+            self._collect_noise(x)
+        C, n = x.shape
+        ptr, stride = None, 0
+        if n > 0:
+            xd, stride, _ = site.kernel_rows(x, self._dtype)
+            ptr = xd.data_ptr()
+        cap = n + self.chunk_size
+        out = site.empty((C, cap), self._kdt)
+        m = self._gate.stream_push(ptr, n, stride, True, out.data_ptr(), cap, cap, site.stream)
+        self._received += n
+        self._returned += m
+        return self._result(out, m)
+
     def finish(self):
         """The rest of the result (fewer than chunk_size + padding samples per channel, or the whole recording when it
         is at most chunk_size samples long); the stream is closed afterwards."""
@@ -177,12 +276,16 @@ class NoiseReduceStream:
         if self._received == 0:
             # what reduce_noise() raises on an empty recording (the reference's _amp_to_db)
             raise ValueError("zero-size array to reduction operation maximum which has no identity")
-        if self._need_thresholds:                   # a recording shorter than chunk_size: thresholds from all of it
-            self._set_stream_thresholds(self._received)
-        dev = samples_for_device(np.empty((1, 0), self._dtype)).dtype
         C = 1 if self.n_channels is None else self.n_channels
         cap = self.chunk_size + self.padding
-        out = np.empty((C, cap), dtype=dev)
-        m = self._gate.stream_finish(out.ctypes.data, cap, cap)
-        self._returned += m
-        return self._result(out, m)
+        with self._on_device():
+            if self._need_thresholds:               # a recording shorter than chunk_size: thresholds from all of it
+                self._set_stream_thresholds(self._received)
+            if self._site is None:
+                out = np.empty((C, cap), dtype=self._kdt)
+                m = self._gate.stream_finish(out.ctypes.data, cap, cap)
+            else:
+                out = self._site.empty((C, cap), self._kdt)
+                m = self._gate.stream_finish(out.data_ptr(), cap, cap, self._site.stream)
+            self._returned += m
+            return self._result(out, m)
