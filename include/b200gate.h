@@ -48,7 +48,18 @@ enum { B200GATE_F32 = 0, B200GATE_I16 = 1, B200GATE_F64 = 2 };     /* sample dty
 enum { B200GATE_BOOL = 3, B200GATE_I8 = 4, B200GATE_U8 = 5, B200GATE_U16 = 6, B200GATE_I32 = 7, B200GATE_U32 = 8,
        B200GATE_I64 = 9, B200GATE_U64 = 10, B200GATE_F16 = 11 };
 enum { B200GATE_CONVERT_CAST = 0, B200GATE_CONVERT_CHANNEL_MEAN = 1 };   /* b200gate_convert operations */
-enum { B200GATE_SURFACE_NUMPY = 0, B200GATE_SURFACE_TORCH = 1 };   /* which reference semantics */
+/* which reference semantics.  NUMPY: SpectralGate's chunk loop (reduce_noise()).  TORCH: TorchGate.forward on whole rows.
+ * TORCH_CHUNKED: reduce_noise(use_torch=True), i.e. the chunk loop of base.py:167-226 around TorchGate
+ * (streamed_torch_gate.py:81-88).  Each (chunk, channel) unit is the padded chunk [i cs - pad, (i + 1) cs + pad), zeros
+ * outside [0, N), filtered with TorchGate's arithmetic (torch.stft(center=True) framing with the window of
+ * b200gate_set_window, per-unit self statistics or the thresholds of b200gate_torch_set_noise, the blend before the
+ * smoothing, the moving-mean follower), always in float64 like the reference's float64 chunks; the run writes columns
+ * [pad, pad + cs) of each unit's torch-length output ((Lp / hop) * hop + (n_fft & 1) samples, Lp = cs + 2 pad).
+ * chunk_size <= 0 (or N <= chunk_size) makes the whole recording one padded chunk [-pad, N + pad).  Ranges and streams
+ * work as on the numpy surface.  Refused with B200GATE_ERR_ARG: a padded chunk shorter than 2 win_length ("x must be
+ * bigger than ..."), and a chunked run whose torch output is shorter than pad + chunk_size.  A single padded chunk whose
+ * torch output is shorter than pad + N writes only its first (torch length - pad) columns, as the reference's slice does. */
+enum { B200GATE_SURFACE_NUMPY = 0, B200GATE_SURFACE_TORCH = 1, B200GATE_SURFACE_TORCH_CHUNKED = 2 };
 
 /* Resolved operator parameters.  The Python shims resolve defaults exactly as the reference does
  * (win_length = n_fft, hop_length = win_length // 4, n_grad_* from Hz / ms) and raise the
@@ -139,11 +150,12 @@ int b200gate_set_noise_threshold(b200gate_handle* h, const double* thresh_db, in
 int b200gate_get_noise_threshold(const b200gate_handle* h, double* thresh_db, int32_t n_bins);
 int b200gate_get_noise_mean_std(const b200gate_handle* h, double* mean_db, double* std_db, int32_t n_bins);
 
-/* Torch surface only: install the analysis/synthesis window the caller built with
+/* Torch surfaces only: install the analysis/synthesis window the caller built with
  * torch.hann_window (float32, win_length values), so tables match the reference bit for bit. */
 int b200gate_set_window(b200gate_handle* h, const float* window, int32_t win_length);
-/* Torch surface only: thresholds from a noise clip xn [Bn][Ln] (float32; Bn == 1 or Bn == batch), as
- * TorchGate.forward(x, xn) (torchgate.py:140-164).  xn == NULL returns to self-statistics. */
+/* Torch surfaces only: thresholds from a noise clip xn [Bn][Ln] (float32; float64 on the general family; Bn == 1 or
+ * Bn == C, the rows of a run), as TorchGate.forward(x, xn) (torchgate.py:140-164).  On TORCH_CHUNKED unit
+ * (chunk, channel) uses row `channel`.  xn == NULL returns to self-statistics. */
 int b200gate_torch_set_noise(b200gate_handle* h, const void* xn, int dtype, int64_t Bn, int64_t Ln,
                              int64_t stride, int is_device, void* cuda_stream);
 
@@ -172,7 +184,7 @@ int b200gate_run(b200gate_handle* h, const void* in, void* out, int dtype, int64
  * written densely into a [C][range] slab (noisereduce_b200/parallel.py gathers such slabs across GPUs). */
 int b200gate_set_range(b200gate_handle* h, int32_t mode, int64_t a, int64_t b);
 
-/* ---- streaming: a recording that arrives block by block (numpy surface, chunk_size > 0) ----------------------------
+/* ---- streaming: a recording that arrives block by block (numpy or TORCH_CHUNKED surface, chunk_size > 0) ----------
  * The reference holds the whole [C][N] input and writes the result to a temp-file memmap (base.py:181-187).  A stream
  * returns each chunk as soon as its padded span has arrived, and the concatenation of everything it returns is
  * bit-identical to b200gate_run on the concatenated input.  Output chunk i (samples [i cs, (i + 1) cs)) reads only input
@@ -192,7 +204,8 @@ int b200gate_set_range(b200gate_handle* h, int32_t mode, int64_t a, int64_t b);
  * before anything is written; a stationary gate without noise thresholds (b200gate_noise_stats /
  * b200gate_set_noise_threshold, which may be called while the stream is open) when a chunk would be returned:
  * B200GATE_ERR_STATE.  While a stream is open b200gate_run on the handle returns B200GATE_ERR_STATE.  After any other
- * error the stream is closed. */
+ * error the stream is closed.  On TORCH_CHUNKED every unit can take its own statistics, so no thresholds are needed;
+ * the single padded chunk of a recording of R <= chunk_size samples may return fewer than R samples (see the surface). */
 int b200gate_stream_begin(b200gate_handle* h, int dtype, int64_t C);
 int b200gate_stream_push(b200gate_handle* h, const void* in, int64_t n, int64_t in_stride, int is_device,
                          void* out, int64_t out_stride, int64_t out_capacity, int64_t* n_out, void* cuda_stream);

@@ -18,7 +18,7 @@ DEFAULT_LIB = os.path.join(_HERE, "libb200gate.so")
 ABI_VERSION = 1
 OK, ERR_ARG, ERR_CUDA, ERR_STATE, ERR_NOMEM = 0, -1, -2, -3, -4
 F32, I16, F64 = 0, 1, 2
-SURFACE_NUMPY, SURFACE_TORCH = 0, 1
+SURFACE_NUMPY, SURFACE_TORCH, SURFACE_TORCH_CHUNKED = 0, 1, 2
 _DTYPES = {np.dtype(np.float32): F32, np.dtype(np.int16): I16, np.dtype(np.float64): F64}
 # b200gate_convert's further formats (include/b200gate.h)
 BOOL, I8, U8, U16, I32, U32, I64, U64, F16 = 3, 4, 5, 6, 7, 8, 9, 10, 11

@@ -22,6 +22,8 @@ struct GGeom {
     int N, logN, W, F;      // n_fft, log2 (power-of-two n_fft), frame length (win_length; n_fft on the torch surface), N/2 + 1
     int M, logM;            // n_fft not a power of two: Bluestein length M = 2^logM >= 2 N - 1 (else 0)
     long long out_len;      // > 0: samples written per row (torch surface: (L / H) * H); 0: the chunk centre
+    long long crop;         // > 0 (chunked torch surface): the chunk centre is cut to the unit's torch output length
+                            // minus the padding, as the reference's slice of a short TorchGate output is
 };
 
 struct GTables {
@@ -180,6 +182,8 @@ struct GDecideArgs {
     double top_db, p;
     const double* thr;      // [thr_units][F] dB (thr_units 1: shared by every unit)
     int thr_units;
+    int thr_rows;           // > 0: unit ul reads row (thr_u0 + ul) % thr_rows (the noise clip's rows are channels)
+    long long thr_u0;
     const unsigned long long* rowmax;
     double* M;              // dB in, mask0 * p + (1 - p) out
     int dbg_ul, FW;
@@ -193,7 +197,8 @@ __global__ void __launch_bounds__(256) gk_decide(const GDecideArgs a) {
         const long long r = i - (long long)ul * TF;
         const int t = (int)(r / a.F), f = (int)(r - (long long)t * a.F);
         const double fl = gk_unord(a.rowmax[(size_t)ul * a.F + f]) - a.top_db;
-        const double th = a.thr[(size_t)(a.thr_units == 1 ? 0 : ul) * a.F + f];
+        const long long tr = a.thr_units == 1 ? 0 : (a.thr_rows > 0 ? (a.thr_u0 + ul) % a.thr_rows : ul);
+        const double th = a.thr[(size_t)tr * a.F + f];
         const bool on = fmax(a.M[i], fl) > th;                               // utils.py:16, stationary.py:99-106
         a.M[i] = (on ? 1.0 : 0.0) * a.p + (1.0 - a.p);                       // stationary.py:108-110
         if (ul == a.dbg_ul && on) atomicOr(a.dbg_bits + (size_t)t * a.FW + (f >> 5), 1u << (f & 31));
@@ -345,7 +350,8 @@ __global__ void __launch_bounds__(256) gk_ola(const GOlaArgs<T> a) {
     const int u = g.u0 + ul;
     const long long chunk = u / g.C, ch = u - chunk * g.C;
     const long long start = chunk * g.step;
-    const long long out_len = a.gg.out_len > 0 ? a.gg.out_len : min((long long)g.step, (long long)(g.n_total - start));
+    long long out_len = a.gg.out_len > 0 ? a.gg.out_len : min((long long)g.step, (long long)(g.n_total - start));
+    if (a.gg.crop > 0) out_len = min(out_len, a.gg.crop);
     const long long sig_len = (long long)(g.T - 1) * H + (W & 1);           // istft length after the boundary crop
     T* yrow = a.y + ch * g.out_stride + start;
     const double* fr = a.frames + (size_t)ul * g.T * W;

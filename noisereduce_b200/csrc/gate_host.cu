@@ -393,7 +393,7 @@ int noise_stats_from_mean(b200gate_handle* h, const double* d_yn, long long n, c
 // ---- general-geometry family: tables, noise statistics ----------------------------------------------------------
 int build_generic_tables(b200gate_handle* h) {
     const int N = h->p.n_fft, W = h->p.win_length;
-    const bool torch_sem = h->p.surface == B200GATE_SURFACE_TORCH;
+    const bool torch_sem = h->p.surface != B200GATE_SURFACE_NUMPY;
     std::vector<double> w(W);
     double sw = 0.0;
     for (int n = 0; n < W; ++n) {
@@ -852,7 +852,8 @@ int b200gate_create(const b200gate_params* p, b200gate_handle** out) {
     *out = nullptr;
     if (p->abi_version != B200GATE_ABI_VERSION)
         return fail(nullptr, B200GATE_ERR_ARG, "ABI version %d, library is %d", p->abi_version, B200GATE_ABI_VERSION);
-    if (p->surface != B200GATE_SURFACE_NUMPY && p->surface != B200GATE_SURFACE_TORCH)
+    if (p->surface != B200GATE_SURFACE_NUMPY && p->surface != B200GATE_SURFACE_TORCH &&
+        p->surface != B200GATE_SURFACE_TORCH_CHUNKED)
         return fail(nullptr, B200GATE_ERR_ARG, "unknown surface %d", p->surface);
     const bool geo1k = p->n_fft == kN && p->win_length == kN && p->hop_length == kN / 4;
     const bool geo2k = p->n_fft == kN2 && p->win_length == kN2 && p->hop_length == kN2 / 4 &&
@@ -862,7 +863,9 @@ int b200gate_create(const b200gate_params* p, b200gate_handle** out) {
     // ... and so does a smoothing filter beyond what the tuned integer kernels hold (16-bit mask numerators, 64 taps a side)
     const bool big_filter = p->n_grad_freq > 64 || p->n_grad_time > 64 ||
                             (long long)(p->n_grad_freq + 1) * (p->n_grad_freq + 1) * (p->n_grad_time + 1) * (p->n_grad_time + 1) > 65535;
-    const bool want_generic = (!geo1k && !geo2k) || (p->path_flags & 4) || big_filter;
+    // the chunked torch surface always runs it: the reference feeds TorchGate float64 chunks (base.py:140)
+    const bool want_generic = (!geo1k && !geo2k) || (p->path_flags & 4) || big_filter ||
+                              p->surface == B200GATE_SURFACE_TORCH_CHUNKED;
     int logN = 0;
     while ((1 << logN) < p->n_fft) ++logN;
     if (want_generic) {
@@ -880,7 +883,7 @@ int b200gate_create(const b200gate_params* p, b200gate_handle** out) {
     if (p->padding < 0) return fail(nullptr, B200GATE_ERR_ARG, "padding must be >= 0");
     // TorchGate asserts 0 <= prop_decrease <= 1 (torchgate.py:52); reduce_noise() takes any value (stationary.py:108)
     if (!std::isfinite(p->prop_decrease) ||
-        (p->surface == B200GATE_SURFACE_TORCH && !(p->prop_decrease >= 0.0 && p->prop_decrease <= 1.0)))
+        (p->surface != B200GATE_SURFACE_NUMPY && !(p->prop_decrease >= 0.0 && p->prop_decrease <= 1.0)))
         return fail(nullptr, B200GATE_ERR_ARG, "prop_decrease must be finite (and in [0, 1] on the torch surface)");
     int ndev = 0;
     cudaError_t e = cudaGetDeviceCount(&ndev);
@@ -1214,7 +1217,7 @@ int b200gate_get_stats(const b200gate_handle* h, b200gate_stats* out) {
 int b200gate_torch_set_noise(b200gate_handle* h, const void* xn, int dtype, int64_t Bn, int64_t Ln, int64_t stride,
                              int is_device, void* stream) {
     if (!h) return B200GATE_ERR_ARG;
-    if (h->p.surface != B200GATE_SURFACE_TORCH) return fail(h, B200GATE_ERR_STATE, "torch surface only");
+    if (h->p.surface == B200GATE_SURFACE_NUMPY) return fail(h, B200GATE_ERR_STATE, "torch surfaces only");
     if (!xn) { h->tthr_units = 0; return B200GATE_OK; }
     const bool f64 = dtype == B200GATE_F64 && h->generic;            // float64 noise clips: general family only
     if (Bn <= 0 || Ln <= 0 || (dtype != B200GATE_F32 && !f64))
@@ -1287,14 +1290,17 @@ int b200gate_torch_set_noise(b200gate_handle* h, const void* xn, int dtype, int6
 static int run_core(b200gate_handle* h, const void* in, void* out, int dtype, int64_t C, int64_t N, int64_t in_stride,
                     int64_t out_stride, int is_device, void* stream, int64_t in_first) {
     if (!h || !in || !out || C <= 0 || N <= 0 || dtype_size(dtype) == 0) return fail(h, B200GATE_ERR_ARG, "bad argument");
-    const bool torch_sem = h->p.surface == B200GATE_SURFACE_TORCH;
-    // torch.istft(center=True) length: n_fft + hop (T - 1) minus n_fft/2 at both ends (torchgate.py:255-262)
-    const int64_t No = torch_sem ? (N / h->p.hop_length) * h->p.hop_length + (h->p.n_fft & 1) : N;
+    // torch_sem: TorchGate's arithmetic; torch_rows: TorchGate.forward on whole rows (no chunk grid, no ranges)
+    const bool torch_sem = h->p.surface != B200GATE_SURFACE_NUMPY;
+    const bool torch_rows = h->p.surface == B200GATE_SURFACE_TORCH;
+    // torch.istft(center=True) length of an L-sample row: n_fft + hop (T - 1) minus n_fft/2 at both ends (torchgate.py:255-262)
+    auto torch_len = [&](long long L) { return (L / h->p.hop_length) * h->p.hop_length + (h->p.n_fft & 1); };
+    const int64_t No = torch_rows ? torch_len(N) : N;
     // In a range mode only samples [o_lo, o_hi) of a row are addressed, so `out` may be a virtual base
     // (slab - o_lo) over rows as short as the range: the stride check below uses the range length.
-    if (in_stride < N - in_first || (out_stride < No && (torch_sem || h->range_mode == 0)))
+    if (in_stride < N - in_first || (out_stride < No && (torch_rows || h->range_mode == 0)))
         return fail(h, B200GATE_ERR_ARG, "row strides too small");
-    if (torch_sem && N < 2 * h->p.win_length) return fail(h, B200GATE_ERR_ARG, "x must be bigger than %d", 2 * h->p.win_length);
+    if (torch_rows && N < 2 * h->p.win_length) return fail(h, B200GATE_ERR_ARG, "x must be bigger than %d", 2 * h->p.win_length);
     if (torch_sem && h->tthr_units > 1 && h->tthr_units != C)
         return fail(h, B200GATE_ERR_ARG, "xn has %d rows, x has %lld", h->tthr_units, (long long)C);
     if (h->p.stationary && !torch_sem && !h->have_thresh)
@@ -1302,30 +1308,38 @@ static int run_core(b200gate_handle* h, const void* in, void* out, int dtype, in
     cudaStream_t st = (cudaStream_t)stream;
     const b200gate_params& p = h->p;
     const size_t es = dtype_size(dtype);
-    h->stats = b200gate_stats{};
-    long long launches = 0;
-    if (!h->reuse_masks) h->masks_valid = false;
 
     // ---- which part of the recording (base.py:167-226; b200gate_set_range) -----------------------------
     // range_mode 2: the reference's single padded chunk [0, a) inside a longer recording (base.py:222)
-    const bool single_to = !torch_sem && h->range_mode == 2;
+    const bool single_to = !torch_rows && h->range_mode == 2;
     if (single_to && h->range_a > N) return fail(h, B200GATE_ERR_ARG, "range end %lld beyond the recording", h->range_a);
-    const bool chunked = !torch_sem && !single_to && p.chunk_size > 0 && N > p.chunk_size;
+    const bool chunked = !torch_rows && !single_to && p.chunk_size > 0 && N > p.chunk_size;
     const long long step = chunked ? p.chunk_size : (single_to ? h->range_a : N);
     const long long n_chunks = chunked ? (N - 1) / p.chunk_size + 1 : 1;
+    // the padded unit TorchGate filters: at least 2 win_length samples (torchgate.py:214-220); on the chunk grid its torch
+    // output must hold the centre of a whole chunk (the reference's slice assignment fails otherwise, base.py:200-207)
+    const long long unit_len = step + (torch_rows ? 0 : 2 * p.padding);
+    if (torch_sem && !torch_rows && unit_len < 2 * p.win_length)
+        return fail(h, B200GATE_ERR_ARG, "x must be bigger than %d", 2 * p.win_length);
+    if (torch_sem && chunked && torch_len(unit_len) - p.padding < step)
+        return fail(h, B200GATE_ERR_ARG, "could not broadcast: a padded chunk of %lld samples gives %lld torch output "
+                    "samples, fewer than padding + chunk_size = %lld", unit_len, torch_len(unit_len), p.padding + step);
+    h->stats = b200gate_stats{};
+    long long launches = 0;
+    if (!h->reuse_masks) h->masks_valid = false;
     // range_mode 1: a sub-range of the chunk grid
     long long chunk_first = 0, chunk_count = n_chunks;
-    if (!torch_sem && h->range_mode == 1) {
+    if (!torch_rows && h->range_mode == 1) {
         if (!chunked || h->range_b >= n_chunks) return fail(h, B200GATE_ERR_ARG, "chunk range outside the chunk grid");
         chunk_first = h->range_a;
         chunk_count = h->range_b - h->range_a + 1;
     }
     // samples written [o_lo, o_hi) and samples read [w_lo, w_hi)
     const long long o_lo = chunk_first * step;
-    const long long o_hi = torch_sem ? No : std::min<long long>(N, (chunk_first + chunk_count) * step);
-    const long long rpad = torch_sem ? 0 : p.padding;
-    const long long w_lo = torch_sem ? 0 : std::max(0LL, o_lo - rpad);
-    const long long w_hi = torch_sem ? N : std::min<long long>(N, o_hi + rpad);
+    const long long o_hi = torch_rows ? No : std::min<long long>(N, (chunk_first + chunk_count) * step);
+    const long long rpad = torch_rows ? 0 : p.padding;
+    const long long w_lo = torch_rows ? 0 : std::max(0LL, o_lo - rpad);
+    const long long w_hi = torch_rows ? N : std::min<long long>(N, o_hi + rpad);
     const long long Wn = w_hi - w_lo, On = o_hi - o_lo;
     if (out_stride < On) return fail(h, B200GATE_ERR_ARG, "output row stride %lld shorter than the range (%lld samples)",
                                      (long long)out_stride, On);
@@ -1391,7 +1405,7 @@ static int run_core(b200gate_handle* h, const void* in, void* out, int dtype, in
     g.n_total = N;
     g.step = step;
     g.n_chunks = (int)n_chunks;
-    g.pad = torch_sem ? 0 : p.padding;                 // TorchGate filters the whole row, no chunk padding
+    g.pad = torch_rows ? 0 : p.padding;                // TorchGate.forward filters the whole row, no chunk padding
     g.Lp = g.step + 2 * g.pad;
     g.T = generic ? (int)((g.Lp + 2 * (h->g_W / 2) - h->g_W) / g.H) + 1 : (int)(g.Lp / g.H) + 1;
     g.in_stride = xs;
@@ -1641,7 +1655,8 @@ static int run_core(b200gate_handle* h, const void* in, void* out, int dtype, in
 
         if (generic) {
             GGeom gg = generic_geom(h, g);
-            if (torch_sem) gg.out_len = No;                 // torch.istft length (torchgate.py:255-262)
+            if (torch_rows) gg.out_len = No;                // torch.istft length (torchgate.py:255-262)
+            else if (torch_sem) gg.crop = torch_len(g.Lp) - g.pad;   // the unit's torch output from column pad on
             const GTables gt = generic_tables(h);
             const int F = h->F, W = h->g_W, FW = (F + 31) / 32;
             double2* gX = (double2*)h->d_ws_buf;
@@ -1671,9 +1686,11 @@ static int run_core(b200gate_handle* h, const void* in, void* out, int dtype, in
                 da.thr = h->d_gthr; da.thr_units = 1; da.rowmax = gRmax;
                 da.M = gM; da.dbg_ul = dbg.ul; da.FW = FW; da.dbg_bits = h->d_dbg_bits;
                 if (torch_sem) {                        // torchgate.py:127-165: per-row statistics (own frames or xn's)
-                    if (h->tthr_units > 0) {
-                        da.thr = h->tthr_units == 1 ? h->d_gtthr : h->d_gtthr + (size_t)u0 * F;
-                        da.thr_units = h->tthr_units == 1 ? 1 : nu;
+                    if (h->tthr_units > 0) {                // xn's rows are channels: unit (chunk, ch) reads row ch
+                        da.thr = h->d_gtthr;
+                        da.thr_units = h->tthr_units;
+                        da.thr_rows = (int)C;
+                        da.thr_u0 = g.u0;
                     } else {
                         double* gThr = (double*)(h->d_ws_buf + goff_thr);
                         GTStatArgs ta{};
@@ -1723,7 +1740,7 @@ static int run_core(b200gate_handle* h, const void* in, void* out, int dtype, in
                 ia.gg = gg; ia.tb = gt; ia.X = gX; ia.M = gM; ia.frames = gFr; ia.dbg_ul = dbg.ul;
                 ia.dbg_spec = (float2*)h->d_dbg_spec; ia.dbg_mask = h->d_dbg_mask;
                 B200_LAUNCH(gk_istft, dim3((unsigned)g.T, (unsigned)nu), dim3(thr_fft), smem_fft, st, ia);
-                const long long out_max = torch_sem ? No : std::min<long long>(g.step, N);
+                const long long out_max = torch_rows ? No : std::min<long long>(g.step, N);
                 B200_WITH_DTYPE(kdt, {
                     GOlaArgs<T> oa{};
                     oa.gg = gg; oa.tb = gt; oa.frames = gFr; oa.y = (T*)yb;
@@ -2230,6 +2247,12 @@ int stream_emit(b200gate_handle* h, long long E_new, bool last, void* out, long 
     return B200GATE_OK;
 }
 
+// a stationary numpy-surface stream needs thresholds before it returns a chunk; the torch surfaces can always take each
+// unit's own statistics
+bool stream_needs_thresholds(const b200gate_handle* h) {
+    return h->p.stationary && h->p.surface == B200GATE_SURFACE_NUMPY && !h->have_thresh;
+}
+
 int stream_check_space(b200gate_handle* h, int is_device) {
     if (!h->s_open) return fail(h, B200GATE_ERR_STATE, "no open stream (b200gate_stream_begin first)");
     if (h->s_is_device >= 0 && h->s_is_device != (is_device ? 1 : 0))
@@ -2242,7 +2265,8 @@ int stream_check_space(b200gate_handle* h, int is_device) {
 int b200gate_stream_begin(b200gate_handle* h, int dtype, int64_t C) {
     if (!h) return B200GATE_ERR_ARG;
     h->s_open = false;
-    if (h->p.surface != B200GATE_SURFACE_NUMPY) return fail(h, B200GATE_ERR_ARG, "streaming needs the numpy surface");
+    if (h->p.surface == B200GATE_SURFACE_TORCH)
+        return fail(h, B200GATE_ERR_ARG, "streaming needs the numpy or the chunked torch surface");
     if (h->p.chunk_size <= 0)
         return fail(h, B200GATE_ERR_ARG, "streaming needs chunk_size > 0 (without chunks nothing can be returned early)");
     const size_t es = dtype_size(dtype);
@@ -2283,7 +2307,7 @@ int b200gate_stream_push(b200gate_handle* h, const void* in, int64_t n, int64_t 
         return fail(h, B200GATE_ERR_ARG, "out_capacity %lld < n + chunk_size = %lld", (long long)out_capacity,
                     (long long)(n + p.chunk_size));
     const long long E0 = h->s_E, E_end = stream_emitted(p, h->s_R + n);
-    if (E_end > E0 && p.stationary && !h->have_thresh)
+    if (E_end > E0 && stream_needs_thresholds(h))
         return fail(h, B200GATE_ERR_STATE, "stationary stream: set the noise thresholds before the first chunk is returned");
     *n_out = E_end - E0;
     if (n == 0) return B200GATE_OK;
@@ -2336,12 +2360,17 @@ int b200gate_stream_finish(b200gate_handle* h, void* out, int64_t out_stride, in
         return fail(h, B200GATE_ERR_ARG, "out_capacity %lld < chunk_size + padding = %lld", (long long)out_capacity,
                     (long long)(p.chunk_size + p.padding));
     const long long E0 = h->s_E, R = h->s_R;
-    if (R > E0 && p.stationary && !h->have_thresh)
+    if (R > E0 && stream_needs_thresholds(h))
         return fail(h, B200GATE_ERR_STATE, "stationary stream: set the noise thresholds before the first chunk is returned");
     rc = stream_emit(h, R, true, out, out_stride, E0, h->s_is_device > 0, (cudaStream_t)stream);
     h->s_open = false;
     if (rc) return rc;
     *n_out = R - E0;
+    // chunked torch surface: a recording of one padded chunk returns what its torch output holds past the padding
+    if (p.surface == B200GATE_SURFACE_TORCH_CHUNKED && R <= p.chunk_size) {
+        const long long Lp = R + 2 * p.padding;
+        *n_out = std::min<long long>(R, (Lp / p.hop_length) * p.hop_length + (p.n_fft & 1) - p.padding);
+    }
     return B200GATE_OK;
 }
 

@@ -32,10 +32,11 @@ def reduce_noise(
     dtype.  ``n_jobs``, ``tmp_folder`` and ``use_tqdm`` are accepted and ignored: the chunk loop they
     steer in the reference runs as one GPU grid here.  ``use_torch=True`` takes the reference's torch route
     (noisereduce.py:121-143 -> StreamedTorchGate): every padded chunk through TorchGate -- a different gate from
-    the numpy one (torch.stft framing, per-chunk self statistics, top_db 40, moving-mean follower; see
-    spectralgate/streamed_torch_gate.py) -- on ``device``, which must be a CUDA device.  There is no CPU path.
+    the numpy one (torch.stft framing, per-chunk self statistics, top_db 40, moving-mean follower, float64 like the
+    reference's chunks; see spectralgate/streamed_torch_gate.py) -- as one GPU grid on ``device``, which must be a CUDA
+    device.  There is no CPU path.
 
-    y may also be a torch CUDA tensor (use_torch=False): the samples are read where they are and the result is a tensor
+    y may also be a torch CUDA tensor, on either route: the samples are read where they are and the result is a tensor
     on the same device, with the same shape and dtype and the same bits as
     ``torch.from_numpy(reduce_noise(y.cpu().numpy(), sr, ...))``.  The work runs on that device's current torch stream,
     but the call does not return with it in flight.  The stationary threshold computation waits for the device.  So
@@ -43,7 +44,8 @@ def reduce_noise(
     other streams (spectralgate/base.py has the details).  ``y_noise`` may
     then be a numpy array, a CPU tensor or a CUDA tensor on y's device (another device raises ValueError).  float16,
     integer and bool tensors are promoted to float64 and cast back on the device with numpy's rules; bfloat16 raises
-    TypeError.  CPU tensors take the numpy route and return numpy arrays, as before.  See spectralgate/base.py.
+    TypeError.  CPU tensors take the numpy route and return numpy arrays, as before.  See spectralgate/base.py.  With
+    use_torch=True and a CUDA y, ``device`` left at "cuda" means y's device; another device raises ValueError.
     """
     if use_torch:
         if n_jobs != 1:                                         # noisereduce.py:115-118

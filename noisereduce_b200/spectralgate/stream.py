@@ -55,16 +55,37 @@ class NoiseReduceStream:
     the stream length or block sizes.  Not supported: chunk_size=None (the whole recording is one unit, so nothing could
     be returned early) and the stationary gate with clip_noise_stationary=False and no y_noise (its thresholds need the
     whole recording); both raise ValueError, as do blocks whose channel count or dtype differ from the first block and a
-    push() after finish().  The torch route (use_torch), TorchGate and multi-GPU streaming are not covered.
+    push() after finish().
+
+    ``use_torch=True`` streams reduce_noise(use_torch=True) -- every chunk through TorchGate's arithmetic in float64 (see
+    spectralgate/streamed_torch_gate.py) -- with the same argument mapping, including that n_std_thresh_stationary is
+    not forwarded.  No noise clip is collected: without y_noise each chunk takes its own statistics, so the stationary
+    gate needs neither y_noise nor clip_noise_stationary.  One more rule: that route clips a y_noise longer than the
+    recording to the recording when clip_noise_stationary, and a stream does not know the recording's length.  So with
+    y_noise and clip_noise_stationary=True the stream returns nothing until len(y_noise) samples have arrived, or until
+    finish(); after that it follows E(R).  ``device`` is where the work runs: "cuda" (the default) means the blocks'
+    device, or the current device for host blocks; a CUDA block on another device than an explicit ``device`` raises
+    ValueError.  Without use_torch, ``device`` is ignored, as in reduce_noise().  TorchGate (the nn.Module) and
+    multi-GPU streaming are not covered.
     """
 
     def __init__(self, sr, n_channels=None, stationary=False, y_noise=None, prop_decrease=1.0, time_constant_s=2.0,
                  freq_mask_smooth_hz=500, time_mask_smooth_ms=50, thresh_n_mult_nonstationary=2,
                  sigmoid_slope_nonstationary=10, n_std_thresh_stationary=1.5, chunk_size=600000, padding=30000,
-                 n_fft=1024, win_length=None, hop_length=None, clip_noise_stationary=True):
+                 n_fft=1024, win_length=None, hop_length=None, clip_noise_stationary=True, use_torch=False,
+                 device="cuda"):
         if chunk_size is None:
             raise ValueError("NoiseReduceStream needs a chunk_size: with chunk_size=None the whole recording is one "
                              "unit and nothing can be returned before the end")
+        if use_torch:
+            self._init_torch(sr, n_channels, stationary, y_noise, prop_decrease, time_constant_s, freq_mask_smooth_hz,
+                             time_mask_smooth_ms, thresh_n_mult_nonstationary, sigmoid_slope_nonstationary,
+                             chunk_size, padding, n_fft, win_length, hop_length, clip_noise_stationary, device)
+            return
+        self._torch = False
+        self._want_device = None
+        self._noise_len = self._hold_until = self._held_n = 0
+        self._held = []
         if stationary and y_noise is None and not clip_noise_stationary:
             raise ValueError("NoiseReduceStream: the stationary gate with clip_noise_stationary=False takes its "
                              "thresholds from the whole recording; pass y_noise or clip_noise_stationary=True")
@@ -119,8 +140,112 @@ class NoiseReduceStream:
             if noise is not None:
                 self._thresh = install_noise_thresholds(self._gate, params, noise, self._clip_to, self._stream())[2]
 
+    def _init_torch(self, sr, n_channels, stationary, y_noise, prop_decrease, time_constant_s, freq_mask_smooth_hz,
+                    time_mask_smooth_ms, thresh_n_mult_nonstationary, sigmoid_slope_nonstationary, chunk_size, padding,
+                    n_fft, win_length, hop_length, clip_noise_stationary, device):
+        """use_torch=True: reduce_noise(use_torch=True)'s argument mapping (noisereduce.py:121-143, with
+        n_std_thresh_stationary not forwarded) onto the chunked torch surface.  Every chunk takes its own statistics,
+        or y_noise's thresholds; no noise clip is collected."""
+        import torch
+        from .streamed_torch_gate import torch_route_params
+        from ..torchgate import TorchGate
+        if n_channels is not None and int(n_channels) < 1:
+            raise ValueError("n_channels must be >= 1 (or None for 1-D blocks)")
+        geo = SpectralGate(np.zeros(1, np.float32), sr, prop_decrease, chunk_size, padding, n_fft, win_length,
+                           hop_length, time_constant_s, freq_mask_smooth_hz, time_mask_smooth_ms, None, False, 1)
+        tg = TorchGate(sr=sr, nonstationary=not stationary, n_thresh_nonstationary=thresh_n_mult_nonstationary,
+                       temp_coeff_nonstationary=1 / sigmoid_slope_nonstationary,
+                       n_movemean_nonstationary=int(time_constant_s / geo._hop_length * sr), prop_decrease=prop_decrease,
+                       n_fft=geo._n_fft, win_length=geo._win_length, hop_length=geo._hop_length,
+                       freq_mask_smooth_hz=freq_mask_smooth_hz, time_mask_smooth_ms=time_mask_smooth_ms)
+        self._torch = True
+        self._tg_win = tg.win_length
+        self._want_device = torch.device(device)
+        if self._want_device.type != "cuda":
+            raise ValueError("noisereduce_b200 has no CPU path: device must be a CUDA device")
+        self.sr = sr
+        self.n_channels = None if n_channels is None else int(n_channels)
+        self.stationary = bool(stationary)
+        self.chunk_size, self.padding = int(chunk_size), int(padding)
+        self._params = torch_route_params(tg, stationary, chunk_size, padding)
+        self._clip_to = None
+        self._dtype = self._kdt = self._site = None
+        self._received = self._returned = 0
+        self._closed = False
+        self._clip = None
+        self._need_thresholds = False
+        self._thresh = None
+        self._gate_device = None
+        # y_noise: TorchGate's xn.  The route clips it to the recording when clip_noise_stationary, so a stream holds
+        # everything back until it has len(y_noise) samples (or finishes) and only then knows the clip.
+        self._xn = None
+        self._held = []
+        self._noise_len = self._hold_until = self._held_n = 0
+        if y_noise is not None:
+            if is_device_tensor(y_noise):
+                self._site = DeviceSite(y_noise)                    # the blocks must then be on y_noise's device
+                if self._want_device.index is not None and self._want_device != self._site.device:
+                    raise ValueError(f"y_noise is on {self._site.device}, device={device!r}")
+            self._xn = y_noise if isinstance(y_noise, torch.Tensor) else np.asarray(y_noise)
+            if clip_noise_stationary:
+                self._noise_len = self._hold_until = int(self._xn.shape[-1])
+        if self._site is not None:
+            self._gate_device = self._site.device
+        elif self._want_device.index is not None:
+            self._gate_device = self._want_device
+        elif torch.cuda.is_initialized():
+            self._gate_device = torch.device("cuda", torch.cuda.current_device())
+        with self._on_device():
+            self._gate = self._new_gate()
+            if self._hold_until == 0:
+                self._release_noise(None)
+
+    def _new_gate(self):
+        """A handle for this stream's parameters, with the thresholds known so far."""
+        if not self._torch:
+            gate = _cabi.Gate(**self._params)
+            if self._thresh is not None:
+                gate.set_noise_threshold(self._thresh)
+            return gate
+        from .streamed_torch_gate import install_torch_noise, make_torch_route_gate
+        gate = make_torch_route_gate(self._params)
+        if self._thresh is not None:                       # (the released, clipped y_noise rows)
+            install_torch_noise(gate, self._thresh, self._noise_device(), self._stream())
+        return gate
+
+    def _noise_device(self):
+        """Where the handle lives, so where install_torch_noise puts y_noise's rows."""
+        torch = sys.modules["torch"]
+        if self._site is not None:
+            return self._site.device
+        if _cabi.library().simulated_device:
+            return torch.device("cpu")
+        if self._want_device.index is not None:
+            return self._want_device
+        return torch.device("cuda", torch.cuda.current_device())
+
+    def _release_noise(self, n_total):
+        """use_torch: y_noise clipped to a recording of n_total samples (None: not clipped) is now known: TorchGate's
+        checks, and the stationary gate's thresholds from it."""
+        self._hold_until = 0
+        if self._xn is None:
+            return
+        from .streamed_torch_gate import check_torch_noise, install_torch_noise, torch_noise_rows
+        xn = self._xn
+        if n_total is not None and xn.shape[-1] > n_total:
+            xn = xn[..., :n_total]
+        xn = torch_noise_rows(xn)
+        check_torch_noise(xn, self._tg_win)
+        if self.stationary:
+            self._thresh = xn
+            install_torch_noise(self._gate, xn, self._noise_device(), self._stream())
+
     def _on_device(self):
-        return contextlib.nullcontext() if self._site is None else self._site.active()
+        if self._site is not None:
+            return self._site.active()
+        if self._want_device is not None and self._want_device.index is not None:
+            return sys.modules["torch"].cuda.device(self._want_device)
+        return contextlib.nullcontext()
 
     def _stream(self):
         return None if self._site is None else self._site.stream
@@ -128,13 +253,15 @@ class NoiseReduceStream:
     # -- emission rule --------------------------------------------------------------------------------------------
     def emitted(self, received=None):
         """E(R): how many samples have been returned once R (default: all pushed so far) have been received."""
-        R = self._received if received is None else int(received)
+        R = self.samples_received if received is None else int(received)
         cs = self.chunk_size
+        if R < self._noise_len:                  # use_torch: held back until y_noise's length is known to be final
+            return 0
         return cs * max(0, (R - self.padding) // cs) if R > cs else 0
 
     @property
     def samples_received(self):
-        return self._received
+        return self._received + self._held_n
 
     @property
     def samples_returned(self):
@@ -180,13 +307,14 @@ class NoiseReduceStream:
         that is not known (torch had not initialised CUDA when the stream was constructed), is remade there once, with
         y_noise's thresholds copied over rather than recomputed; closing the old handle waits for the device."""
         if self._site is None:
+            want = self._want_device
+            if want is not None and want.index is not None and want != x.device:
+                raise ValueError(f"this block is on {x.device}, the stream's device is {want}")
             self._site = DeviceSite(x)
         if self._site.cuda and self._gate_device != self._site.device:
             self._gate.close()
             with self._site.active():
-                self._gate = _cabi.Gate(**self._params)
-                if self._thresh is not None:
-                    self._gate.set_noise_threshold(self._thresh)
+                self._gate = self._new_gate()
         self._gate_device = self._site.device
 
     def _collect_noise(self, x):
@@ -232,6 +360,29 @@ class NoiseReduceStream:
         returns a CUDA tensor; the call only enqueues work on the device's current torch stream, except when it
         completes the stationary noise clip (the thresholds are read back once)."""
         x = self._rows(block)
+        if self._hold_until:
+            x = self._hold(x)
+            if x is None:
+                return self._result(np.empty((1 if self.n_channels is None else self.n_channels, 0), self._kdt), 0)
+        return self._push_rows(x)
+
+    def _hold(self, x):
+        """use_torch with a y_noise that the route would clip to the recording: keep the blocks (copied: the caller may
+        reuse its buffers) until len(y_noise) samples have arrived; then return them all as one block."""
+        self._held.append(x.clone() if self._site is not None else np.array(x))
+        self._held_n += x.shape[1]
+        if self._received + self._held_n < self._hold_until:
+            return None
+        return self._take_held(None)
+
+    def _take_held(self, n_total):
+        held, self._held, self._held_n = self._held, [], 0
+        x = sys.modules["torch"].cat(held, dim=1) if self._site is not None else np.concatenate(held, axis=1)
+        with self._on_device():
+            self._release_noise(n_total)
+        return x
+
+    def _push_rows(self, x):
         if self._site is not None:
             with self._site.active():
                 return self._push_device(x)
@@ -272,10 +423,19 @@ class NoiseReduceStream:
         is at most chunk_size samples long); the stream is closed afterwards."""
         if self._closed:
             raise ValueError("finish() after finish(): the stream is closed")
-        self._closed = True
-        if self._received == 0:
+        if self.samples_received == 0:
+            self._closed = True
             # what reduce_noise() raises on an empty recording (the reference's _amp_to_db)
             raise ValueError("zero-size array to reduction operation maximum which has no identity")
+        if self._held_n:                # use_torch: y_noise is clipped to the recording, which is complete now
+            head = self._push_rows(self._take_held(self.samples_received))
+            tail = self._finish_rows()
+            cat = sys.modules["torch"].cat if self._site is not None else np.concatenate
+            return cat([head, tail], -1)
+        return self._finish_rows()
+
+    def _finish_rows(self):
+        self._closed = True
         C = 1 if self.n_channels is None else self.n_channels
         cap = self.chunk_size + self.padding
         with self._on_device():
