@@ -725,6 +725,15 @@ static void launch_smooth_float(SmoothFArgs sa, int nf, int nt, int tf_lo, int t
     }
 }
 
+// k_iir_sigmoid may rebuild its forward sweep by the inverse recurrence (IirArgs::regen) only where the bound on the
+// relative error of the follower S that this costs, 2.5 u (1-b)^(-2T) / b with u = 2^-53 (derived at k_iir_sigmoid),
+// stays within 2^-24, the float32 rounding the stored forward sweep puts on S:  2 T ln(1/(1-b)) - ln b <= 29 ln 2 - ln 2.5.
+// (Config 3, 48 kHz / n_fft 2048 / 600000-sample chunks: T = 1290, b = 0.00532 -> 19.00 of 19.19.)
+static int iir_regen_ok(double b, int T, int path_flags) {
+    if (path_flags & 64 || !(b < 0.5)) return 0;
+    return 2.0 * (double)T * -log1p(-b) - log(b) <= 29.0 * log(2.0) - log(2.5) ? 1 : 0;
+}
+
 // Pageable host memory: cudaMemcpyAsync from / to it is neither asynchronous nor fast (the driver bounces it through a small
 // pinned buffer at ~10 GB/s), and pinning a caller's 7 GB array in place costs a second (measured: cudaHostRegister 8.5 GB/s).
 // The slab pipeline therefore stages pageable rows through its own pinned slabs with a handful of host threads
@@ -1968,7 +1977,7 @@ static int run_core(b200gate_handle* h, const void* in, void* out, int dtype, in
                     ia.b = (sqrt(1.0 + 4.0 * tfr * tfr) - 1.0) / (2.0 * tfr * tfr);
                 }
                 ia.n_mult = (float)p.thresh_n_mult; ia.slope = (float)p.sigmoid_slope;
-                ia.regen = (ia.b < 0.5 && (double)g.T * -log1p(-ia.b) < 20.0 && !(p.path_flags & 64)) ? 1 : 0;
+                ia.regen = iir_regen_ok(ia.b, g.T, p.path_flags);
                 ia.mag = d_mag; ia.m0 = d_m0;
                 B200_LAUNCH(k_iir_sigmoid<kFPad2>, dim3(grid_1d((long long)nu * kFPad2, 128, 1 << 30)), dim3(128), 0, st, ia);
                 launches += 2;
@@ -2027,7 +2036,7 @@ static int run_core(b200gate_handle* h, const void* in, void* out, int dtype, in
                         ia.b = (sqrt(1.0 + 4.0 * tfr * tfr) - 1.0) / (2.0 * tfr * tfr);
                     }
                     ia.n_mult = (float)p.thresh_n_mult; ia.slope = (float)p.sigmoid_slope;
-                ia.regen = (ia.b < 0.5 && (double)g.T * -log1p(-ia.b) < 20.0 && !(p.path_flags & 64)) ? 1 : 0;
+                    ia.regen = iir_regen_ok(ia.b, g.T, p.path_flags);
                     ia.mag = d_mag; ia.m0 = d_m0;
                     B200_LAUNCH(k_iir_sigmoid<kFPad>, dim3(grid_1d((long long)nu * kFPad, 128, 1 << 30)), dim3(128), 0, st, ia);
                 }

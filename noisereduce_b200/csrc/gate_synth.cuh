@@ -324,38 +324,64 @@ __global__ void __launch_bounds__(kThreads, B200_K2C_MINBLOCKS) k2c_synthesize(c
                         if (vb) a.dbg.mask[(long long)(t + 1) * kF + k] = 2.0f * mb;
                     }
                 }
-                // ---- lower pairs k = lane + 32 q < 512: both members -------------------------------------------
+                // Float masks: a non-finite value in one frame's row would reach its partner through s and d (both
+                // frames share Z).  The apply below notes any non-finite s; only then (a warp vote per pair) is the
+                // offending frame found, its row zeroed in this warp's buffer, the apply redone and the frame's whole
+                // overlap-add span made NaN after the transform -- the reference's istft of a NaN row.  Finite masks
+                // take one pass and the very same arithmetic as before.
+                bool nan_a = false, nan_b = false;
+#pragma unroll 1
+                for (int pass = 0;; ++pass) {
+                    bool bad = false;
+                    // ---- lower pairs k = lane + 32 q < 512: both members -------------------------------------------
 #pragma unroll
-                for (int q = 0; q < 16; ++q) {
-                    const int k = 32 * q + lane;
-                    const float2 own = zbuf[k];
-                    const float2 par = zbuf[q == 0 ? ((kN - lane) & (kN - 1)) : (kN - k)];
-                    float ma, mb;
-                    half_masks(k, ma, mb);
-                    const float s = ma + mb, d = ma - mb;
-                    // Z'[k] = s Z[k] + d conj(Z[N-k]);  Z'[N-k] = s Z[N-k] + d conj(Z[k])
-                    im[q] = fmaf(d, par.x, s * own.x);
-                    re[q] = fmaf(-d, par.y, s * own.y);
-                    const float qr = fmaf(d, own.x, s * par.x), qi = fmaf(-d, own.y, s * par.y);
-                    qbuf[512 - k] = make_float2(qi, qr);                 // slot of bin N - k, stored (re, im) as the FFT wants them
-                }
-                {   // slot 16: bins 512 + lane, computed directly (lane 0 = the self-mirrored bin N/2)
-                    const float2 own = zbuf[512 + lane];
-                    const float2 par = zbuf[512 - lane];
-                    float ma, mb;
-                    half_masks(512 - lane, ma, mb);
-                    const float s = ma + mb, d = ma - mb;
-                    im[16] = fmaf(d, par.x, s * own.x);
-                    re[16] = fmaf(-d, par.y, s * own.y);
-                }
-                __syncwarp();
+                    for (int q = 0; q < 16; ++q) {
+                        const int k = 32 * q + lane;
+                        const float2 own = zbuf[k];
+                        const float2 par = zbuf[q == 0 ? ((kN - lane) & (kN - 1)) : (kN - k)];
+                        float ma, mb;
+                        half_masks(k, ma, mb);
+                        const float s = ma + mb, d = ma - mb;
+                        if (MK == kMaskF32) bad |= !(fabsf(s) < INFINITY);
+                        // Z'[k] = s Z[k] + d conj(Z[N-k]);  Z'[N-k] = s Z[N-k] + d conj(Z[k])
+                        im[q] = fmaf(d, par.x, s * own.x);
+                        re[q] = fmaf(-d, par.y, s * own.y);
+                        const float qr = fmaf(d, own.x, s * par.x), qi = fmaf(-d, own.y, s * par.y);
+                        qbuf[512 - k] = make_float2(qi, qr);             // slot of bin N - k, stored (re, im) as the FFT wants them
+                    }
+                    {   // slot 16: bins 512 + lane, computed directly (lane 0 = the self-mirrored bin N/2)
+                        const float2 own = zbuf[512 + lane];
+                        const float2 par = zbuf[512 - lane];
+                        float ma, mb;
+                        half_masks(512 - lane, ma, mb);
+                        const float s = ma + mb, d = ma - mb;
+                        if (MK == kMaskF32) bad |= !(fabsf(s) < INFINITY);
+                        im[16] = fmaf(d, par.x, s * own.x);
+                        re[16] = fmaf(-d, par.y, s * own.y);
+                    }
+                    __syncwarp();
 #pragma unroll
-                for (int q = 17; q < 32; ++q) {
-                    const float2 v = qbuf[32 * (q - 16) + lane];
-                    re[q] = v.x;
-                    im[q] = v.y;
+                    for (int q = 17; q < 32; ++q) {
+                        const float2 v = qbuf[32 * (q - 16) + lane];
+                        re[q] = v.x;
+                        im[q] = v.y;
+                    }
+                    __syncwarp();
+                    if (MK != kMaskF32 || pass > 0 || !__any_sync(0xffffffffu, bad)) break;
+                    float* mw = reinterpret_cast<float*>(mbuf);
+                    bool ba = false, bb = false;
+                    for (int k = lane; k < kF; k += 32) {
+                        ba |= !(fabsf(mw[k]) < INFINITY);
+                        bb |= !(fabsf(mw[kFPad + k]) < INFINITY);
+                    }
+                    nan_a = __any_sync(0xffffffffu, ba);
+                    nan_b = vb && __any_sync(0xffffffffu, bb);
+                    for (int k = lane; k < kF; k += 32) {
+                        if (nan_a) mw[k] = 0.f;
+                        if (nan_b) mw[kFPad + k] = 0.f;
+                    }
+                    __syncwarp();
                 }
-                __syncwarp();
                 if (t + 2 <= t_last) stage(t + 2);           // next pair streams in behind this pair's transform
 #if B200_K2C_PTW
                 warp_fft1024_ptw(re, im, tile, s_tw4, lane);
@@ -363,6 +389,13 @@ __global__ void __launch_bounds__(kThreads, B200_K2C_MINBLOCKS) k2c_synthesize(c
                 warp_fft1024(re, im, tile, s_tw, lane);
 #endif
                 // now im = N a'[n], re = N b'[n] (n = lane + 32 q) at slot brev5(q)
+                if (MK == kMaskF32 && (nan_a || nan_b)) {
+#pragma unroll
+                    for (int q = 0; q < 32; ++q) {
+                        if (nan_a) im[q] = __uint_as_float(0x7fc00000u);
+                        if (nan_b) re[q] = __uint_as_float(0x7fc00000u);
+                    }
+                }
 #pragma unroll
                 for (int q = 0; q < 32; ++q) {
                     const float w = s_ws[lane + 32 * q];
