@@ -184,6 +184,35 @@ int b200gate_run(b200gate_handle* h, const void* in, void* out, int dtype, int64
  * written densely into a [C][range] slab (noisereduce_b200/parallel.py gathers such slabs across GPUs). */
 int b200gate_set_range(b200gate_handle* h, int32_t mode, int64_t a, int64_t b);
 
+/* ---- the adjoint: backpropagation through b200gate_run (numpy surface) ---------------------------------------------
+ * With its masks held fixed (the thresholds, decisions, top_db row flags and the non-stationary noise floor are
+ * constants, as in TorchGate's backward, torchgate.py:223-262), unit u = (chunk i, channel c) of a run is a linear map of
+ * its padded span: y_u = crop(D^-1 OLA(w P w frame(pad_u y))), P = irfft diag(M) rfft cut to the frame (a symmetric
+ * matrix), D = sum of w^2 (1 where <= 1e-10).  b200gate_adjoint computes grad = A^T g, the sum over units of the same
+ * re-transforming synthesis run on g / D over the unit's centre (zero elsewhere, including centre samples the forward
+ * leaves at zero), with an un-normalised overlap-add over the whole padded span [i cs - pad, (i + 1) cs + pad) clipped to
+ * [0, N).  Spans of overlapping units are added in increasing unit order without atomics: the result is the same in every
+ * bit from run to run and for any workspace limit.
+ *
+ * b200gate_mask_store_bytes: the size of the masks a run of [C][N] keeps, in the handle's current range mode.
+ * b200gate_set_mask_store: a caller-owned device buffer of `bytes` bytes (NULL: keep nothing, the default).  While it is
+ *   set, each b200gate_run writes its final masks there instead of to the workspace -- the same kernels and the same
+ *   bits, no extra traffic: stationary n_fft 1024, the decision words and top_db row flags (68 B per frame and unit); the
+ *   non-stationary gate (n_fft 1024 and 2048), the float masks; the general family, the float64 masks.  A run whose masks do not
+ *   fit returns B200GATE_ERR_ARG.  Streams never keep masks.
+ * b200gate_adjoint: grad [C][N] (row stride grad_stride, every sample written) = A^T g for the run whose masks are in
+ *   `store` (same C, N and range mode as that run; B200GATE_ERR_STATE otherwise).  g is read on the samples the run
+ *   wrote only, so in range modes 1 and 2 it may be a virtual base like `out` (g_stride >= the range length).  dtype
+ *   B200GATE_F32 or B200GATE_F64 for both g and grad (the n_fft 2048 kernels read float32 rows: a float64 g is converted
+ *   through the handle's staging buffer); device pointers only (is_device = 1); enqueued on cuda_stream.
+ *   The adjoint grows the handle's workspace as a run does (the per-unit span and numerators, within the workspace
+ *   limit); it stays allocated until the handle is destroyed.
+ * All three refuse the torch surfaces (B200GATE_ERR_STATE; their backward is b200gate_torch_apply_masks). */
+int b200gate_mask_store_bytes(b200gate_handle* h, int64_t C, int64_t N, int64_t* bytes);
+int b200gate_set_mask_store(b200gate_handle* h, void* store, int64_t bytes);
+int b200gate_adjoint(b200gate_handle* h, const void* store, const void* g, void* grad, int dtype, int64_t C, int64_t N,
+                     int64_t g_stride, int64_t grad_stride, int is_device, void* cuda_stream);
+
 /* ---- streaming: a recording that arrives block by block (numpy or TORCH_CHUNKED surface, chunk_size > 0) ----------
  * The reference holds the whole [C][N] input and writes the result to a temp-file memmap (base.py:181-187).  A stream
  * returns each chunk as soon as its padded span has arrived, and the concatenation of everything it returns is

@@ -37,6 +37,7 @@ EXPORTS = [
     "b200gate_run_sharded", "b200gate_peer_push", "b200gate_peer_barrier", "b200gate_torch_apply_masks",
     "b200gate_host_alloc", "b200gate_host_free",
     "b200gate_stream_begin", "b200gate_stream_push", "b200gate_stream_finish", "b200gate_convert",
+    "b200gate_mask_store_bytes", "b200gate_set_mask_store", "b200gate_adjoint",
 ]
 
 
@@ -127,6 +128,9 @@ class GateLibrary:
         d.b200gate_stream_push.argtypes = [vp, vp, i64, i64, C.c_int, vp, i64, i64, C.POINTER(i64), vp]
         d.b200gate_stream_finish.argtypes = [vp, vp, i64, i64, C.POINTER(i64), vp]
         d.b200gate_convert.argtypes = [C.c_int, vp, C.c_int, i64, vp, C.c_int, i64, i64, i64, vp]
+        d.b200gate_mask_store_bytes.argtypes = [vp, i64, i64, C.POINTER(i64)]
+        d.b200gate_set_mask_store.argtypes = [vp, vp, i64]
+        d.b200gate_adjoint.argtypes = [vp, vp, vp, vp, C.c_int, i64, i64, i64, i64, C.c_int, vp]
 
 
 def format_code(dt) -> int:
@@ -330,6 +334,19 @@ class Gate:
     def torch_apply_masks_device(self, in_ptr, out_ptr, dtype, C_, N, in_stride, out_stride, stream=None):
         self._check(self.lib.dll.b200gate_torch_apply_masks(
             self._h, in_ptr, out_ptr, dtype_code(dtype), C_, N, in_stride, out_stride, 1, stream))
+
+    # -- kept masks and the adjoint (numpy surface) ---------------------------------------------------------------------
+    def mask_store_bytes(self, C_, N) -> int:
+        n = C.c_int64()
+        self._check(self.lib.dll.b200gate_mask_store_bytes(self._h, C_, N, C.byref(n)))
+        return n.value
+
+    def set_mask_store(self, ptr, nbytes=0):
+        self._check(self.lib.dll.b200gate_set_mask_store(self._h, ptr, nbytes))
+
+    def adjoint_device(self, store_ptr, g_ptr, grad_ptr, dtype, C_, N, g_stride, grad_stride, stream=None):
+        self._check(self.lib.dll.b200gate_adjoint(self._h, store_ptr, g_ptr, grad_ptr, dtype_code(dtype), C_, N, g_stride,
+                                                  grad_stride, 1, stream))
 
     # -- streaming (b200gate_stream_*): pointers and sizes as in the header; the push / finish return n_out --------------
     def stream_begin(self, dtype, C_):

@@ -109,7 +109,21 @@ struct GStftArgs {
     const T* x;
     double2* X;             // [n_units][T][F]
 };
-template <typename T>
+// sum of w^2 over the frames overlapping padded-chunk index i (gk_ola's normaliser; 1 where it is <= 1e-10)
+__device__ __forceinline__ double gk_norm(const GGeom& gg, const GTables& tb, long long i) {
+    const int W = gg.W, H = gg.g.H;
+    const long long j = i + W / 2;
+    long long t_lo = (j - W + H) / H;
+    if (j - W + 1 <= 0) t_lo = 0;
+    const long long t_hi = min((long long)(gg.g.T - 1), j / H);
+    double nrm = 0.0;
+    for (long long t = t_lo; t <= t_hi; ++t) nrm += tb.w2[(int)(j - t * H)];
+    return nrm > 1e-10 ? nrm : 1.0;
+}
+
+// ADJ (b200gate_adjoint): x is the gradient of the output; the frames read it on the unit's centre only, divided by
+// the overlap-add norm, and zero elsewhere (the adjoint of gk_ola's normalise-and-crop)
+template <typename T, bool ADJ = false>
 __global__ void __launch_bounds__(256) gk_stft(const GStftArgs<T> a) {
     B200_DYN_SMEM(double2, s);
     const Geom& g = a.gg.g;
@@ -121,9 +135,17 @@ __global__ void __launch_bounds__(256) gk_stft(const GStftArgs<T> a) {
     const T* xrow = a.x + ch * g.in_stride;
     const long long base = (long long)t * g.H - W / 2;            // boundary='zeros': W/2 zeros either side
     const int len = gk_len(a.gg);
+    long long c_hi = 0;                                            // ADJ: end of the centre the forward writes
+    if (ADJ) {
+        c_hi = g.pad + min((long long)g.step, (long long)(g.n_total - chunk * g.step));
+        c_hi = min(c_hi, (long long)(g.T - 1) * g.H + (W & 1));
+    }
     for (int n = threadIdx.x; n < len; n += blockDim.x) {
         double v = 0.0;
-        if (n < W) v = chunk_sample_f64(xrow, base + n, i1, g.Lp, g.n_total) * a.tb.wa[n];
+        if (ADJ) {
+            const long long j = base + n;
+            if (n < W && j >= g.pad && j < c_hi) v = ld_sample_f64(xrow + i1 + j) / gk_norm(a.gg, a.tb, j) * a.tb.wa[n];
+        } else if (n < W) v = chunk_sample_f64(xrow, base + n, i1, g.Lp, g.n_total) * a.tb.wa[n];
         const double2 z = n < N ? gk_in(a.gg, a.tb, n, make_double2(v, 0.0)) : make_double2(0.0, 0.0);
         s[n < N ? gk_slot(a.gg, n) : n] = z;                      // rfft(n=N): zero-padded at the end
     }
@@ -341,12 +363,28 @@ struct GOlaArgs {
     GTables tb;
     const double* frames;
     T* y;
+    double* adj;            // ADJ: [n_units][adj_pitch], the un-normalised overlap-add of the padded span [0, Lp)
+    long long adj_pitch;
 };
-template <typename T>
+template <typename T, bool ADJ = false>
 __global__ void __launch_bounds__(256) gk_ola(const GOlaArgs<T> a) {
     const Geom& g = a.gg.g;
     const int W = a.gg.W, H = g.H;
     const int ul = blockIdx.y;
+    if (ADJ) {
+        double* arow = a.adj + (size_t)ul * a.adj_pitch;
+        const double* fr = a.frames + (size_t)ul * g.T * W;
+        for (long long i = (long long)blockIdx.x * blockDim.x + threadIdx.x; i < g.Lp; i += (long long)gridDim.x * blockDim.x) {
+            const long long j = i + W / 2;
+            long long t_lo = (j - W + H) / H;
+            if (j - W + 1 <= 0) t_lo = 0;
+            const long long t_hi = min((long long)(g.T - 1), j / H);
+            double acc = 0.0;
+            for (long long t = t_lo; t <= t_hi; ++t) acc += fr[(size_t)t * W + (int)(j - t * H)];
+            arow[i] = acc;
+        }
+        return;
+    }
     const int u = g.u0 + ul;
     const long long chunk = u / g.C, ch = u - chunk * g.C;
     const long long start = chunk * g.step;

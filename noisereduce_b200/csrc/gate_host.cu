@@ -12,6 +12,7 @@
 #include "gate_peer.cuh"
 #include "gate_generic.cuh"
 #include "gate_convert.cuh"
+#include "gate_adjoint.cuh"
 
 #include <math.h>
 #include <cmath>
@@ -88,6 +89,14 @@ struct b200gate_handle {
     // with the same masks, TorchGate.backward) can reuse them -- b200gate_torch_apply_masks
     bool masks_valid = false, reuse_masks = false;
     long long masks_C = 0, masks_N = 0;
+    // numpy surface: b200gate_set_mask_store's caller-owned buffer.  While it is set, b200gate_run carves the buffers
+    // its kernels write the final masks to from it (every unit of the call) instead of from the workspace, and records
+    // which run the store holds, so that b200gate_adjoint can check it is handed masks of its own geometry.
+    void* mask_store = nullptr;
+    int64_t mask_store_bytes = 0;
+    bool keep_masks = false;                       // this b200gate_run keeps its masks in mask_store
+    struct KeptRun { const void* store; long long C, N, a, b; int mode; size_t bytes; };
+    std::vector<KeptRun> kept;                     // the stores filled by earlier runs (most recent last)
     bool stats_pending = false;
     size_t pend_batches = 0;
     std::vector<cudaEvent_t> group_ev;             // b200gate_run_sharded: one per channel group + 1
@@ -695,6 +704,39 @@ static void set_k2c_smoothing_taps(K2Args& a, int nf) {
     memcpy(a.sm_taps, tb8, sizeof tb8);
 }
 
+// Stationary gate: the integer mask numerators of frames [sa.tf_lo, sa.tf_hi) from the decisions and row flags
+// (k_smooth_packed where the byte lanes hold the filter, else k_smooth_generic).  `sa` carries the unit count, frames,
+// filter extents, TT and the three buffers.
+static void launch_stationary_numerators(const b200gate_handle* h, const SmoothArgs& sa, cudaStream_t st) {
+    const int nf = sa.nf, nt = sa.nt, nu = sa.n_units, tf_lo = sa.tf_lo, tf_hi = sa.tf_hi;
+    const int ntaps = 2 * nf + 1;
+    if (packed_smoothing_fits(nf, nt)) {
+        SmoothPArgs pa{};
+        pa.n_units = nu; pa.T = sa.T; pa.nf = nf; pa.nt = nt; pa.tf_lo = tf_lo; pa.tf_hi = tf_hi;
+        pa.bits = sa.bits; pa.rowflag = sa.rowflag; pa.num = sa.num;
+        unsigned char tb8[36] = {0};
+        for (int d = -nf; d <= nf; ++d) tb8[d + nf] = (unsigned char)(nf + 1 - abs(d));
+        memcpy(pa.taps, tb8, 36);
+        // strips: enough CTAs to fill the machine, long enough to amortise the 2 nt warm-up frames
+        const int groups = (nu + kSmoothUnits - 1) / kSmoothUnits;
+        int n_strips = std::max(1, std::min((tf_hi - tf_lo + 127) / 128, (h->num_sm * 4 + groups - 1) / groups));
+        pa.strip = (tf_hi - tf_lo + n_strips - 1) / n_strips;
+        pa.strip = (pa.strip + kSmoothBatch - 1) / kSmoothBatch * kSmoothBatch;     // frame pairs (2j, 2j+1) leave together
+        n_strips = (tf_hi - tf_lo + pa.strip - 1) / pa.strip;
+        const dim3 grid(n_strips, groups);
+        if (ntaps <= 12) {
+            B200_LAUNCH(k_smooth_packed<3>, grid, dim3(kSmoothThreads), smoothp_smem_bytes<3>(), st, pa);
+        } else if (ntaps <= 24) {
+            B200_LAUNCH(k_smooth_packed<6>, grid, dim3(kSmoothThreads), smoothp_smem_bytes<6>(), st, pa);
+        } else {
+            B200_LAUNCH(k_smooth_packed<9>, grid, dim3(kSmoothThreads), smoothp_smem_bytes<9>(), st, pa);
+        }
+    } else {
+        const int tiles = (tf_hi - tf_lo + sa.TT - 1) / sa.TT;
+        B200_LAUNCH(k_smooth_generic, dim3(tiles, nu), dim3(256), smooth_smem_bytes(sa.TT, nf, nt), st, sa);
+    }
+}
+
 // Float-mask smoothing (non-stationary gate, TorchGate moving-mean gate): the box form for 1 <= nf <= 12 (k_smooth_box,
 // compiled per nf), else the tap-loop streaming kernel, else (ring too large for shared memory) the tile kernel.
 #define B200_SMOOTH_BOX_CASE(NF_) case NF_: { auto kern_ = k_smooth_box<NF_>; \
@@ -948,12 +990,20 @@ int b200gate_create(const b200gate_params* p, b200gate_handle** out) {
         cudaFuncSetAttribute(k_smooth_stream, cudaFuncAttributeMaxDynamicSharedMemorySize, 200 * 1024);
         for (int nfb = 1; nfb <= 12; ++nfb) smooth_box_dispatch(SmoothFArgs{}, nfb, dim3(1), 0, nullptr, true);
         cudaFuncSetAttribute(k1n_magnitude_2k, cudaFuncAttributeMaxDynamicSharedMemorySize, k1n2_smem_floats() * 4);
-        cudaFuncSetAttribute(k2_synthesize_2k, cudaFuncAttributeMaxDynamicSharedMemorySize, k22_smem_floats() * 4);
+        cudaFuncSetAttribute(k2_synthesize_2k<>, cudaFuncAttributeMaxDynamicSharedMemorySize, k22_smem_floats() * 4);
+        cudaFuncSetAttribute(k2_synthesize_2k<true>, cudaFuncAttributeMaxDynamicSharedMemorySize, k22_smem_floats() * 4);
         cudaFuncSetAttribute(k2c_synthesize_2k, cudaFuncAttributeMaxDynamicSharedMemorySize, k2c2_smem_bytes());
         cudaFuncSetAttribute(k_smooth_generic, cudaFuncAttributeMaxDynamicSharedMemorySize, 160 * 1024);
         for (int dt = 0; dt < 3; ++dt)
             B200_WITH_DTYPE(dt, { cudaFuncSetAttribute(gk_stft<T>, cudaFuncAttributeMaxDynamicSharedMemorySize, 8192 * 16); });
         cudaFuncSetAttribute(gk_istft, cudaFuncAttributeMaxDynamicSharedMemorySize, 8192 * 16);
+        // the adjoint (b200gate_adjoint): float32 / float64 gradients
+        cudaFuncSetAttribute(k2_synthesize<8, false, float, true>, cudaFuncAttributeMaxDynamicSharedMemorySize, k2_smem_floats(256) * 4);
+        cudaFuncSetAttribute(k2_synthesize<8, true, float, true>, cudaFuncAttributeMaxDynamicSharedMemorySize, k2_smem_floats(256) * 4);
+        cudaFuncSetAttribute(k2_synthesize<8, false, double, true>, cudaFuncAttributeMaxDynamicSharedMemorySize, k2_smem_floats(256) * 4);
+        cudaFuncSetAttribute(k2_synthesize<8, true, double, true>, cudaFuncAttributeMaxDynamicSharedMemorySize, k2_smem_floats(256) * 4);
+        cudaFuncSetAttribute(gk_stft<float, true>, cudaFuncAttributeMaxDynamicSharedMemorySize, 8192 * 16);
+        cudaFuncSetAttribute(gk_stft<double, true>, cudaFuncAttributeMaxDynamicSharedMemorySize, 8192 * 16);
 #endif
     }
     if (rc != B200GATE_OK) {
@@ -1294,6 +1344,91 @@ int b200gate_torch_set_noise(b200gate_handle* h, const void* xn, int dtype, int6
     return B200GATE_OK;
 }
 
+// ---- the chunk grid of a run (base.py:167-226; b200gate_set_range) ---------------------------------------------------
+// One computation serves run_core and the kept-mask layout, so the two cannot disagree on the units or their frames.
+// torch surface (TorchGate.forward on whole rows): one unit per row, no padding, no ranges.
+struct RunGrid {
+    bool single_to = false;       // range mode 2: the reference's single padded chunk [0, a) (base.py:222)
+    bool chunked = false;
+    long long step = 0, n_chunks = 1, first = 0, count = 1, pad = 0, Lp = 0;
+    int T = 0;                    // frames per unit
+};
+
+static int run_grid(b200gate_handle* h, long long N, RunGrid* rg) {
+    const b200gate_params& p = h->p;
+    const bool torch_rows = p.surface == B200GATE_SURFACE_TORCH;
+    *rg = RunGrid{};
+    rg->single_to = !torch_rows && h->range_mode == 2;
+    if (rg->single_to && h->range_a > N) return fail(h, B200GATE_ERR_ARG, "range end %lld beyond the recording", h->range_a);
+    rg->chunked = !torch_rows && !rg->single_to && p.chunk_size > 0 && N > p.chunk_size;
+    rg->step = rg->chunked ? p.chunk_size : (rg->single_to ? h->range_a : N);
+    rg->n_chunks = rg->chunked ? (N - 1) / p.chunk_size + 1 : 1;
+    rg->count = rg->n_chunks;
+    if (!torch_rows && h->range_mode == 1) {                 // a sub-range of the chunk grid
+        if (!rg->chunked || h->range_b >= rg->n_chunks) return fail(h, B200GATE_ERR_ARG, "chunk range outside the chunk grid");
+        rg->first = h->range_a;
+        rg->count = h->range_b - h->range_a + 1;
+    }
+    rg->pad = torch_rows ? 0 : p.padding;                    // TorchGate.forward filters the whole row, no chunk padding
+    rg->Lp = rg->step + 2 * rg->pad;
+    if (rg->Lp / p.hop_length > 0x3fffffffLL) return fail(h, B200GATE_ERR_ARG, "problem too large");
+    rg->T = h->generic ? (int)((rg->Lp + 2 * (h->g_W / 2) - h->g_W) / p.hop_length) + 1 : (int)(rg->Lp / p.hop_length) + 1;
+    return B200GATE_OK;
+}
+
+// ---- kept masks (b200gate_mask_store_bytes / b200gate_set_mask_store / b200gate_adjoint) ----------------------------
+// The layout of the masks a run keeps: every unit of the call in unit order, at a fixed size per unit, so that a batch's
+// buffers sit at its unit offset whatever the batching.
+struct MaskPlan {
+    Geom g;                       // H, C, T, n_chunks, n_total, step, pad, Lp (u0 / n_units are per batch)
+    long long U = 0, Ubase = 0;   // units of the call and its first unit
+    size_t unit_bytes = 0;        // stationary, n_fft 1024: decision words [T][FW]; else the final mask [T][FPad] / [T][F]
+    size_t off_rowflag = 0;       // stationary, n_fft 1024: the top_db row flags [U][FW] follow the decisions
+    size_t bytes = 0;
+};
+
+static bool mask_family_ok(b200gate_handle* h) {
+    if (h->p.surface != B200GATE_SURFACE_NUMPY) {
+        fail(h, B200GATE_ERR_STATE, "kept masks and the adjoint are for the numpy surface (the torch surface's backward "
+                                    "is b200gate_torch_apply_masks)");
+        return false;
+    }
+    return true;
+}
+
+// the store layout of U units of T frames
+static void mask_layout(const b200gate_handle* h, int T, long long U_, MaskPlan* mp) {
+    const size_t U = (size_t)U_;
+    if (h->generic) {
+        mp->unit_bytes = (size_t)T * h->F * sizeof(double);
+        mp->bytes = U * mp->unit_bytes;
+    } else if (h->p.stationary) {
+        mp->unit_bytes = (size_t)T * kFW * 4;
+        mp->off_rowflag = (U * mp->unit_bytes + 255) / 256 * 256;
+        mp->bytes = mp->off_rowflag + U * kFW * 4;
+    } else {
+        mp->unit_bytes = (size_t)T * (h->p.n_fft == kN2 ? kFPad2 : kFPad) * 4;
+        mp->bytes = U * mp->unit_bytes;
+    }
+}
+
+static int mask_plan(b200gate_handle* h, long long C, long long N, MaskPlan* mp) {
+    if (!mask_family_ok(h)) return B200GATE_ERR_STATE;
+    if (C <= 0 || N <= 0) return fail(h, B200GATE_ERR_ARG, "bad argument");
+    RunGrid rg;
+    const int rc = run_grid(h, N, &rg);
+    if (rc) return rc;
+    *mp = MaskPlan{};
+    Geom& g = mp->g;
+    g.H = h->p.hop_length; g.C = (int)C; g.n_total = N; g.n_chunks = (int)rg.n_chunks;
+    g.step = rg.step; g.pad = rg.pad; g.Lp = rg.Lp; g.T = rg.T;
+    mp->U = rg.count * C;
+    mp->Ubase = rg.first * C;
+    if (mp->Ubase + mp->U > 0x7fffffffLL) return fail(h, B200GATE_ERR_ARG, "problem too large");
+    mask_layout(h, g.T, mp->U, mp);
+    return B200GATE_OK;
+}
+
 // b200gate_run on input rows that hold only samples [in_first, N) (a stream's window, addressed through the virtual base
 // `in` = window - in_first): the row stride then only has to cover that span.
 static int run_core(b200gate_handle* h, const void* in, void* out, int dtype, int64_t C, int64_t N, int64_t in_stride,
@@ -1320,11 +1455,14 @@ static int run_core(b200gate_handle* h, const void* in, void* out, int dtype, in
 
     // ---- which part of the recording (base.py:167-226; b200gate_set_range) -----------------------------
     // range_mode 2: the reference's single padded chunk [0, a) inside a longer recording (base.py:222)
-    const bool single_to = !torch_rows && h->range_mode == 2;
-    if (single_to && h->range_a > N) return fail(h, B200GATE_ERR_ARG, "range end %lld beyond the recording", h->range_a);
-    const bool chunked = !torch_rows && !single_to && p.chunk_size > 0 && N > p.chunk_size;
-    const long long step = chunked ? p.chunk_size : (single_to ? h->range_a : N);
-    const long long n_chunks = chunked ? (N - 1) / p.chunk_size + 1 : 1;
+    RunGrid rg;
+    {
+        const int rc = run_grid(h, N, &rg);
+        if (rc) return rc;
+    }
+    const bool chunked = rg.chunked;
+    const long long step = rg.step;
+    const long long n_chunks = rg.n_chunks;
     // the padded unit TorchGate filters: at least 2 win_length samples (torchgate.py:214-220); on the chunk grid its torch
     // output must hold the centre of a whole chunk (the reference's slice assignment fails otherwise, base.py:200-207)
     const long long unit_len = step + (torch_rows ? 0 : 2 * p.padding);
@@ -1337,12 +1475,7 @@ static int run_core(b200gate_handle* h, const void* in, void* out, int dtype, in
     long long launches = 0;
     if (!h->reuse_masks) h->masks_valid = false;
     // range_mode 1: a sub-range of the chunk grid
-    long long chunk_first = 0, chunk_count = n_chunks;
-    if (!torch_rows && h->range_mode == 1) {
-        if (!chunked || h->range_b >= n_chunks) return fail(h, B200GATE_ERR_ARG, "chunk range outside the chunk grid");
-        chunk_first = h->range_a;
-        chunk_count = h->range_b - h->range_a + 1;
-    }
+    const long long chunk_first = rg.first, chunk_count = rg.count;
     // samples written [o_lo, o_hi) and samples read [w_lo, w_hi)
     const long long o_lo = chunk_first * step;
     const long long o_hi = torch_rows ? No : std::min<long long>(N, (chunk_first + chunk_count) * step);
@@ -1414,14 +1547,23 @@ static int run_core(b200gate_handle* h, const void* in, void* out, int dtype, in
     g.n_total = N;
     g.step = step;
     g.n_chunks = (int)n_chunks;
-    g.pad = torch_rows ? 0 : p.padding;                // TorchGate.forward filters the whole row, no chunk padding
-    g.Lp = g.step + 2 * g.pad;
-    g.T = generic ? (int)((g.Lp + 2 * (h->g_W / 2) - h->g_W) / g.H) + 1 : (int)(g.Lp / g.H) + 1;
+    g.pad = rg.pad;
+    g.Lp = rg.Lp;
+    g.T = rg.T;
     g.in_stride = xs;
     g.out_stride = ys;
     const long long U = chunk_count * C;
     const long long Ubase = chunk_first * C;               // first unit of the selected range
     if (Ubase + U > 0x7fffffffLL || g.Lp / g.H > 0x3fffffffLL) return fail(h, B200GATE_ERR_ARG, "problem too large");
+    // kept masks (b200gate_set_mask_store): each batch's mask buffers are carved from the store at its unit offset
+    MaskPlan kp{};
+    const bool keep = h->keep_masks;
+    if (keep) {                                            // (the layout of this very run's units and frames)
+        mask_layout(h, g.T, U, &kp);
+        if ((int64_t)kp.bytes > h->mask_store_bytes)
+            return fail(h, B200GATE_ERR_ARG, "mask store of %lld bytes; this run keeps %zu", (long long)h->mask_store_bytes,
+                        kp.bytes);
+    }
 
     const int NFFT = p.n_fft;
     const bool two_k = NFFT == kN2 && !generic;
@@ -1612,6 +1754,15 @@ static int run_core(b200gate_handle* h, const void* in, void* out, int dtype, in
         const int nu = (int)std::min(ub, U - u0);
         g.u0 = (int)(Ubase + u0);
         g.n_units = nu;
+        if (keep && !generic) {
+            char* ks = (char*)h->mask_store;
+            if (stat) {
+                d_bits = (unsigned*)(ks + (size_t)u0 * kp.unit_bytes);
+                d_rowflag = (unsigned*)(ks + kp.off_rowflag + (size_t)u0 * kFW * 4);
+            } else {
+                d_mag = (float*)(ks + (size_t)u0 * kp.unit_bytes);
+            }
+        }
         const void* xb = x;
         void* yb = y;
         if (pipelined) {
@@ -1669,7 +1820,7 @@ static int run_core(b200gate_handle* h, const void* in, void* out, int dtype, in
             const GTables gt = generic_tables(h);
             const int F = h->F, W = h->g_W, FW = (F + 31) / 32;
             double2* gX = (double2*)h->d_ws_buf;
-            double* gM = (double*)(h->d_ws_buf + goff_M);
+            double* gM = keep ? (double*)((char*)h->mask_store + (size_t)u0 * kp.unit_bytes) : (double*)(h->d_ws_buf + goff_M);
             double* gTmp = (double*)(h->d_ws_buf + goff_tmp);
             double* gFr = (double*)(h->d_ws_buf + goff_fr);
             const int thr_fft = generic_threads(generic_fft_len(h));
@@ -1849,36 +2000,13 @@ static int run_core(b200gate_handle* h, const void* in, void* out, int dtype, in
                 SmoothArgs sa{};
                 sa.n_units = nu; sa.T = g.T; sa.nf = nf; sa.nt = nt; sa.tf_lo = tf_lo; sa.tf_hi = tf_hi; sa.TT = 32;
                 sa.bits = d_bits; sa.rowflag = d_rowflag; sa.num = d_num;
-                const int ntaps = 2 * nf + 1;
                 if (smooth_in_k2) {
                     // k2c_synthesize smooths the decisions itself (they and the row flags stay in the workspace, so the
                     // reuse_masks backward gets the forward's masks too)
                 } else if (h->reuse_masks) {
                     // the numerators of the last forward are still in d_num
-                } else if (packed_smoothing_fits(nf, nt)) {
-                    SmoothPArgs pa{};
-                    pa.n_units = nu; pa.T = g.T; pa.nf = nf; pa.nt = nt; pa.tf_lo = tf_lo; pa.tf_hi = tf_hi;
-                    pa.bits = d_bits; pa.rowflag = d_rowflag; pa.num = d_num;
-                    unsigned char tb8[36] = {0};
-                    for (int d = -nf; d <= nf; ++d) tb8[d + nf] = (unsigned char)(nf + 1 - abs(d));
-                    memcpy(pa.taps, tb8, 36);
-                    // strips: enough CTAs to fill the machine, long enough to amortise the 2 nt warm-up frames
-                    const int groups = (nu + kSmoothUnits - 1) / kSmoothUnits;
-                    int n_strips = std::max(1, std::min((tf_hi - tf_lo + 127) / 128, (h->num_sm * 4 + groups - 1) / groups));
-                    pa.strip = (tf_hi - tf_lo + n_strips - 1) / n_strips;
-                    pa.strip = (pa.strip + kSmoothBatch - 1) / kSmoothBatch * kSmoothBatch;     // frame pairs (2j, 2j+1) leave together
-                    n_strips = (tf_hi - tf_lo + pa.strip - 1) / pa.strip;
-                    const dim3 grid(n_strips, groups);
-                    if (ntaps <= 12) {
-                        B200_LAUNCH(k_smooth_packed<3>, grid, dim3(kSmoothThreads), smoothp_smem_bytes<3>(), st, pa);
-                    } else if (ntaps <= 24) {
-                        B200_LAUNCH(k_smooth_packed<6>, grid, dim3(kSmoothThreads), smoothp_smem_bytes<6>(), st, pa);
-                    } else {
-                        B200_LAUNCH(k_smooth_packed<9>, grid, dim3(kSmoothThreads), smoothp_smem_bytes<9>(), st, pa);
-                    }
                 } else {
-                    const int tiles = (tf_hi - tf_lo + sa.TT - 1) / sa.TT;
-                    B200_LAUNCH(k_smooth_generic, dim3(tiles, nu), dim3(256), smooth_smem_bytes(sa.TT, nf, nt), st, sa);
+                    launch_stationary_numerators(h, sa, st);
                 }
                 cudaEventRecord(h->stage_ev[4 * bi + 2], st);
                 K2Args a2{};
@@ -2011,7 +2139,7 @@ static int run_core(b200gate_handle* h, const void* in, void* out, int dtype, in
                         a2.run = (int)std::max(16LL, std::min(128LL, run));
                         a2.n_runs = (int)((hops + a2.run - 1) / a2.run);
                     }
-                    B200_LAUNCH(k2_synthesize_2k, dim3(grid_1d((long long)nu * a2.n_runs, kWarps, res2)), dim3(kThreads),
+                    B200_LAUNCH(k2_synthesize_2k<>, dim3(grid_1d((long long)nu * a2.n_runs, kWarps, res2)), dim3(kThreads),
                                 k22_smem_floats() * 4, st, a2);
                     }
                     cudaEventRecord(h->stage_ev[4 * bi + 3], st);
@@ -2187,6 +2315,12 @@ static int run_core(b200gate_handle* h, const void* in, void* out, int dtype, in
         h->masks_valid = true; h->masks_C = C; h->masks_N = N;
     }
     h->pend_batches = n_batches;
+    if (keep) {
+        for (size_t i = h->kept.size(); i-- > 0;)
+            if (h->kept[i].store == h->mask_store) h->kept.erase(h->kept.begin() + (long)i);
+        if (h->kept.size() >= 64) h->kept.erase(h->kept.begin());
+        h->kept.push_back({h->mask_store, (long long)C, (long long)N, h->range_a, h->range_b, h->range_mode, kp.bytes});
+    }
     if (!direct) {                               // host buffers: the result must be in `out` on return
         const int rc = resolve_stats(h);
         if (rc) return rc;
@@ -2198,7 +2332,227 @@ static int run_core(b200gate_handle* h, const void* in, void* out, int dtype, in
 int b200gate_run(b200gate_handle* h, const void* in, void* out, int dtype, int64_t C, int64_t N, int64_t in_stride,
                  int64_t out_stride, int is_device, void* stream) {
     if (h && h->s_open) return fail(h, B200GATE_ERR_STATE, "a stream is open on this handle (b200gate_stream_finish first)");
-    return run_core(h, in, out, dtype, C, N, in_stride, out_stride, is_device, stream, 0);
+    if (h) h->keep_masks = h->mask_store != nullptr;
+    const int rc = run_core(h, in, out, dtype, C, N, in_stride, out_stride, is_device, stream, 0);
+    if (h) h->keep_masks = false;
+    return rc;
+}
+
+int b200gate_mask_store_bytes(b200gate_handle* h, int64_t C, int64_t N, int64_t* bytes) {
+    if (!h || !bytes) return B200GATE_ERR_ARG;
+    MaskPlan kp{};
+    const int rc = mask_plan(h, C, N, &kp);
+    if (rc) return rc;
+    *bytes = (int64_t)kp.bytes;
+    return B200GATE_OK;
+}
+
+int b200gate_set_mask_store(b200gate_handle* h, void* store, int64_t bytes) {
+    if (!h) return B200GATE_ERR_ARG;
+    if (store && !mask_family_ok(h)) return B200GATE_ERR_STATE;
+    if (store && bytes <= 0) return fail(h, B200GATE_ERR_ARG, "mask store of %lld bytes", (long long)bytes);
+    h->mask_store = store;
+    h->mask_store_bytes = store ? bytes : 0;
+    return B200GATE_OK;
+}
+
+}  // extern "C"
+
+namespace {
+template <typename T>
+int adjoint_impl(b200gate_handle* h, const MaskPlan& kp, const char* store, const T* gin, T* grad, long long g_stride,
+                 long long grad_stride, cudaStream_t st) {
+    const b200gate_params& p = h->p;
+    const bool generic = h->generic, stat = p.stationary != 0;
+    const bool two_k = !generic && p.n_fft == kN2;             // float32 rows only (as run_core converts at the edge)
+    const long long C = kp.g.C, N = kp.g.n_total, U = kp.U, Ubase = kp.Ubase;
+    Geom g = kp.g;
+    g.in_stride = g_stride;
+    g.out_stride = grad_stride;
+    const void* gk = gin;                                      // g as the synthesis kernel reads it
+    if (two_k && sizeof(T) != sizeof(float)) {
+        // the n_fft 2048 kernels read float32 rows: g's centre samples [o_lo, o_hi) go through the staging buffer
+        const long long o_lo = (Ubase / C) * g.step, o_hi = std::min<long long>(N, (Ubase + U) / C * g.step);
+        const long long On = o_hi - o_lo;
+        int rc;
+        if ((rc = ensure(h, (void**)&h->d_in, &h->in_bytes, (size_t)C * On * sizeof(float)))) return rc;
+        { auto kern_ = k_to_f32<T>;
+          B200_LAUNCH(kern_, dim3(grid_1d(C * On, 256, h->num_sm * 16)), dim3(256), 0, st, gin + o_lo, (float*)h->d_in, C, On,
+                      g_stride, On); }
+        gk = (const float*)h->d_in - o_lo;
+        g.in_stride = On;
+    }
+    // every sample of grad is written: zeros where no unit of the call reads the input
+    if (C == 1 || grad_stride == N)
+        CK(h, cudaMemsetAsync(grad, 0, (size_t)C * N * sizeof(T), st));
+    else
+        for (long long c = 0; c < C; ++c) CK(h, cudaMemsetAsync(grad + c * grad_stride, 0, (size_t)N * sizeof(T), st));
+    // frames whose masks the synthesis applies (run_core's tf_lo / tf_hi and output hops h_lo / h_hi of a full chunk)
+    const int NFFT = p.n_fft;
+    const long long sig_len = (long long)(g.T - 1) * g.H + (generic ? (h->g_W & 1) : 0);
+    const long long jp_hi = std::min(g.pad + g.step, sig_len);
+    if (jp_hi <= g.pad) return B200GATE_OK;                  // no unit writes a sample: the gradient is zero
+    const int h_lo = (int)((g.pad + NFFT / 2) / g.H), h_hi = (int)((jp_hi + NFFT / 2 + g.H - 1) / g.H);
+    const int tf_lo = std::max(0, h_lo - 3) & ~1, tf_hi = std::min(h_hi, g.T);
+    // per-unit workspace: the adjoint's span [0, Lp), plus the numerators (stationary) or the spectra and synthesis
+    // frames (general family)
+    auto al = [](size_t v) { return (v + 255) / 256 * 256; };
+    const size_t g_tf = (size_t)g.T * (size_t)h->F, g_tw = (size_t)g.T * (size_t)h->g_W;
+    const size_t num_bytes = (!generic && stat) ? (size_t)num_unit_stride(g.T) * 2 : 0;
+    const size_t adj_es = generic ? sizeof(double) : sizeof(float);
+    const size_t per_unit = generic ? g_tf * 16 + g_tw * 8 + (size_t)g.Lp * 8 + 3 * 256
+                                    : num_bytes + (size_t)g.Lp * 4 + 2 * 256;
+    double limit = p.workspace_limit_bytes;
+    if (!(limit > 0)) {
+        limit = 24.0 * 1024 * 1024 * 1024;
+        size_t free_b = 0, total_b = 0;
+        if (cudaMemGetInfo(&free_b, &total_b) == cudaSuccess)
+            limit = std::min(limit, 0.7 * ((double)free_b + (double)h->ws_bytes));
+    }
+    long long ub = std::min<long long>(U, (long long)std::max(1.0, floor(limit / (double)per_unit)));
+    if (generic) ub = std::min(ub, 65535LL);
+    for (;;) {
+        if (ensure(h, (void**)&h->d_ws_buf, &h->ws_bytes, (size_t)ub * per_unit + ((size_t)8 << 20)) == B200GATE_OK) break;
+        cudaGetLastError();
+        if (ub / 2 < 1) return B200GATE_ERR_NOMEM;           // (message set by ensure)
+        ub /= 2;
+    }
+    if (ub < U) {                                            // equal batches, as run_core
+        const long long nb = (U + ub - 1) / ub;
+        ub = std::min(ub, (U + nb - 1) / nb);
+    }
+    char* ws = h->d_ws_buf;
+    const size_t off_a = generic ? al((size_t)ub * g_tf * 16) : 0;          // generic: spectra, then frames
+    const size_t off_adj = generic ? off_a + al((size_t)ub * g_tw * 8) : al((size_t)ub * num_bytes);
+    const long long adj_pitch = g.Lp;
+    const int resident = h->num_sm * 3;
+    const Tables tb = device_tables(h);
+    const int nf = p.n_grad_freq, nt = p.n_grad_time;
+    const double D = (double)(nf + 1) * (nf + 1) * (nt + 1) * (nt + 1);
+    for (long long u0 = 0; u0 < U; u0 += ub) {
+        const int nu = (int)std::min(ub, U - u0);
+        g.u0 = (int)(Ubase + u0);
+        g.n_units = nu;
+        if (generic) {
+            const GGeom gg = generic_geom(h, g);
+            const GTables gt = generic_tables(h);
+            double2* gX = (double2*)ws;
+            double* gFr = (double*)(ws + off_a);
+            double* adj = (double*)(ws + off_adj);
+            const int thr_fft = generic_threads(generic_fft_len(h));
+            const size_t smem_fft = (size_t)generic_fft_len(h) * sizeof(double2);
+            GStftArgs<T> sa{};
+            sa.gg = gg; sa.tb = gt; sa.x = gin; sa.X = gX;
+            { auto kern_ = gk_stft<T, true>;
+              B200_LAUNCH(kern_, dim3((unsigned)g.T, (unsigned)nu), dim3(thr_fft), smem_fft, st, sa); }
+            GIstftArgs ia{};
+            ia.gg = gg; ia.tb = gt; ia.X = gX; ia.M = (const double*)(store + (size_t)u0 * kp.unit_bytes); ia.frames = gFr;
+            ia.dbg_ul = -1;
+            B200_LAUNCH(gk_istft, dim3((unsigned)g.T, (unsigned)nu), dim3(thr_fft), smem_fft, st, ia);
+            GOlaArgs<T> oa{};
+            oa.gg = gg; oa.tb = gt; oa.frames = gFr; oa.adj = adj; oa.adj_pitch = adj_pitch;
+            { auto kern_ = gk_ola<T, true>;
+              B200_LAUNCH(kern_, dim3((unsigned)grid_1d(g.Lp, 256, 1 << 16), (unsigned)nu), dim3(256), 0, st, oa); }
+        } else {
+            float* adj = (float*)(ws + off_adj);
+            CK(h, cudaMemsetAsync(adj, 0, (size_t)nu * adj_pitch * adj_es, st));   // hops no frame of the centre reaches
+            K2Args a2{};
+            a2.g = g; a2.tb = tb; a2.x = gin; a2.y = nullptr; a2.zcache = nullptr; a2.nt = nt; a2.dbg.ul = -1;
+            a2.adj = adj; a2.adj_pitch = adj_pitch;
+            if (stat) {
+                unsigned short* num = (unsigned short*)ws;
+                SmoothArgs sa{};
+                sa.n_units = nu; sa.T = g.T; sa.nf = nf; sa.nt = nt; sa.tf_lo = tf_lo; sa.tf_hi = tf_hi; sa.TT = 32;
+                sa.bits = (const unsigned*)(store + (size_t)u0 * kp.unit_bytes);
+                sa.rowflag = (const unsigned*)(store + kp.off_rowflag + (size_t)u0 * kFW * 4);
+                sa.num = num;
+                launch_stationary_numerators(h, sa, st);
+                a2.num = num;
+                a2.pD = (float)(p.prop_decrease / D);
+                a2.one_minus_p = (float)(1.0 - p.prop_decrease);
+            } else {
+                a2.fmask = (const float*)(store + (size_t)u0 * kp.unit_bytes);
+            }
+            // output hops: every hop the frames [h_lo - 3, h_hi - 1] overlap (k2_synthesize<.., ADJ>)
+            const int NH = NFFT / g.H;
+            const long long hops = (std::min(h_hi - 1, g.T - 1) + NH) - std::max(0, h_lo - (NH - 1));
+            const int res_k2 = two_k ? h->num_sm * 2 : resident;
+            long long run = ((long long)nu * hops + (long long)res_k2 * kWarps * 4 - 1) / ((long long)res_k2 * kWarps * 4);
+            run = std::max(16LL, std::min(128LL, run));
+            run += run & 1;
+            a2.run = (int)run;
+            a2.n_runs = (int)((hops + a2.run - 1) / a2.run);
+            const dim3 grid2(grid_1d((long long)nu * a2.n_runs, kWarps, res_k2));
+            if (two_k) {
+                K22Args a22{};
+                a22.g = g; a22.x = (const float*)gk; a22.y = nullptr; a22.fmask = a2.fmask; a22.dbg.ul = -1;
+                a22.tb.wa2 = h->d_wa2; a22.tb.ws2 = h->d_ws2; a22.tb.tw = h->d_tw; a22.tb.w2k = h->d_w2k;
+                a22.tb.invn2 = h->d_invn2; a22.tb.ws_to_w = h->ws_to_w;
+                a22.run = a2.run; a22.n_runs = a2.n_runs; a22.adj = adj; a22.adj_pitch = adj_pitch;
+                B200_LAUNCH(k2_synthesize_2k<true>, grid2, dim3(kThreads), k22_smem_floats() * 4, st, a22);
+            } else if (stat) {
+                auto kern2 = k2_synthesize<8, false, T, true>;
+                B200_LAUNCH(kern2, grid2, dim3(kThreads), k2_smem_floats(g.H) * 4, st, a2);
+            } else {
+                auto kern2 = k2_synthesize<8, true, T, true>;
+                B200_LAUNCH(kern2, grid2, dim3(kThreads), k2_smem_floats(g.H) * 4, st, a2);
+            }
+        }
+        // the ordered sum of this batch's spans into grad
+        const long long cf = g.u0 / C, cl = (g.u0 + nu - 1) / C;
+        const long long s_lo = std::max(0LL, cf * g.step - g.pad), s_hi = std::min<long long>(N, (cl + 1) * g.step + g.pad);
+        // (channels ride on gridDim.y, at most 65535 per launch)
+        for (long long c0 = 0; s_hi > s_lo && c0 < C; c0 += 65535) {
+            const long long nc = std::min(C - c0, 65535LL);
+            const dim3 grid3(grid_1d(s_hi - s_lo, 256, std::max(1, 8192 / (int)std::min<long long>(nc, 8192))), (unsigned)nc);
+            if (generic) {
+                auto kern3 = k_adj_gather<double, T>;
+                B200_LAUNCH(kern3, grid3, dim3(256), 0, st, (const double*)(ws + off_adj), adj_pitch, grad,
+                            (long long)grad_stride, g, s_lo, s_hi, (int)c0);
+            } else {
+                auto kern3 = k_adj_gather<float, T>;
+                B200_LAUNCH(kern3, grid3, dim3(256), 0, st, (const float*)(ws + off_adj), adj_pitch, grad,
+                            (long long)grad_stride, g, s_lo, s_hi, (int)c0);
+            }
+        }
+        CK(h, cudaGetLastError());
+    }
+    return B200GATE_OK;
+}
+}  // namespace
+
+extern "C" {
+
+int b200gate_adjoint(b200gate_handle* h, const void* store, const void* g_in, void* grad, int dtype, int64_t C, int64_t N,
+                     int64_t g_stride, int64_t grad_stride, int is_device, void* stream) {
+    if (!h) return B200GATE_ERR_ARG;
+    MaskPlan kp{};
+    int rc = mask_plan(h, C, N, &kp);
+    if (rc) return rc;
+    if (!store || !g_in || !grad || (dtype != B200GATE_F32 && dtype != B200GATE_F64))
+        return fail(h, B200GATE_ERR_ARG, "b200gate_adjoint: null pointer, or a gradient dtype other than float32 / float64");
+    if (!is_device) return fail(h, B200GATE_ERR_ARG, "b200gate_adjoint takes device pointers");
+    if (h->s_open) return fail(h, B200GATE_ERR_STATE, "a stream is open on this handle (b200gate_stream_finish first)");
+    // the centre the forward wrote, [o_lo, o_hi): g is read there only, so a virtual base over a shorter slab will do
+    const long long o_lo = (kp.Ubase / C) * kp.g.step;
+    const long long o_hi = std::min<long long>(N, (kp.Ubase + kp.U) / C * kp.g.step);
+    if (grad_stride < N || (C > 1 && g_stride < (h->range_mode == 0 ? N : o_hi - o_lo)))
+        return fail(h, B200GATE_ERR_ARG, "row strides too small");
+    const MaskPlan* mp = &kp;
+    bool found = false;
+    for (const auto& r : h->kept)
+        if (r.store == store) {
+            found = r.C == C && r.N == N && r.mode == h->range_mode && r.bytes == mp->bytes &&
+                    (r.mode == 0 || (r.a == h->range_a && (r.mode == 2 || r.b == h->range_b)));
+            break;
+        }
+    if (!found)
+        return fail(h, B200GATE_ERR_STATE, "the mask store holds no masks of a b200gate_run of this handle with C = %lld, "
+                    "N = %lld and the current range", (long long)C, (long long)N);
+    cudaStream_t st = (cudaStream_t)stream;
+    if (dtype == B200GATE_F64)
+        return adjoint_impl<double>(h, kp, (const char*)store, (const double*)g_in, (double*)grad, g_stride, grad_stride, st);
+    return adjoint_impl<float>(h, kp, (const char*)store, (const float*)g_in, (float*)grad, g_stride, grad_stride, st);
 }
 
 // ---- streaming: the recording arrives in blocks (include/b200gate.h) --------------------------------------------------

@@ -849,6 +849,11 @@ struct K2Args {
     int sm_ws;                     // first tap word of bin group i: row word i + sm_ws
     int sm_ntw;                    // tap words (4, 7, 9 or 10)
     unsigned sm_taps[10];          // triangle taps nf+1-|d| as bytes, after (sm_pad - nf) % 4 zero bytes
+    // k2_synthesize<.., ADJ = true>: the adjoint of a unit (b200gate_adjoint).  x is the gradient g of the output,
+    // read on the unit's centre only and divided by the overlap-add norm; the un-normalised overlap-add of the whole
+    // padded span goes to adj[ul][0, Lp) (chunk-local index), which k_adj_gather sums across units.
+    float* adj;
+    long long adj_pitch;
 };
 
 constexpr int k2_smem_floats(int H) { return 2 * kN + 2 * kN + H + kFPad + kWarps * kExchFloats + 8 + kWarps * 2 * kN; }
@@ -861,7 +866,58 @@ __device__ __forceinline__ float time_edge(int t, int T, int nt) {
     return (float)s / (float)((nt + 1) * (nt + 1));
 }
 
-template <int HR, bool FMASK, typename T>
+// 1 / (sum of w^2 over the frames overlapping chunk-local sample jp): the overlap-add norm k2_synthesize divides by
+// (scipy's istft; 1 where the sum is <= 1e-10).  Called for the first and last hops of a unit only: kept out of line so
+// the adjoint's interior frames, which read s_invn, carry none of its registers.
+#ifdef B200_CUSIM_BUILD
+#define B200_NOINLINE
+#else
+#define B200_NOINLINE __noinline__
+#endif
+template <int HR>
+__device__ B200_NOINLINE float k2_edge_inv_norm(long long jp, int H, int T, const float* s_invn, const float* s_ws,
+                                                float ws_to_w) {
+    constexpr int NH = 32 / HR;
+    const long long q = jp + kN / 2;
+    const int hop = (int)(q / H), ro = (int)(q - (long long)hop * H);
+    if (hop >= NH - 1 && hop <= T - 1) return s_invn[ro];
+    float nrm = 0.f;
+    for (int i = 0; i < NH; ++i) {
+        const int tf = hop - i;
+        if (tf >= 0 && tf <= T - 1) {
+            const float w = s_ws[i * H + ro] * ws_to_w;
+            nrm = fmaf(w, w, nrm);
+        }
+    }
+    return nrm > 1e-10f ? 1.0f / nrm : 1.0f;
+}
+
+// The adjoint's input frame pair (t, t+1): g / norm on the unit's centre [pad, jp_hi), zero elsewhere.  Row r of the
+// pair window is row r % HR of hop t + r / HR; when every one of those hops is interior the norm is s_invn's.
+template <int HR, typename T>
+__device__ __forceinline__ float load_adjoint_pair(float (&re)[32], float (&im)[32], const T* __restrict__ grow, int t,
+                                                   long long base, long long i1, long long pad, long long jp_hi, int H,
+                                                   int T_, const float* __restrict__ s_invn,
+                                                   const float* __restrict__ s_ws, float ws_to_w,
+                                                   const float* __restrict__ s_wa, int lane, bool vb) {
+    constexpr int NH = 32 / HR;
+    const bool interior = t >= NH - 1 && t + (32 + HR - 1) / HR <= T_ - 1;
+    float xr[32 + HR];
+#pragma unroll
+    for (int r = 0; r < 32 + HR; ++r) {
+        const long long j = base + lane + 32 * r;
+        float v = 0.0f;
+        if (j >= pad && j < jp_hi) {
+            const float inv = interior ? s_invn[(r % HR) * 32 + lane]
+                                       : k2_edge_inv_norm<HR>(j, H, T_, s_invn, s_ws, ws_to_w);
+            v = ld_sample(grow + i1 + j) * inv;
+        }
+        xr[r] = v;
+    }
+    return pack_frame_pair<HR>(re, im, xr, s_wa, lane, vb);
+}
+
+template <int HR, bool FMASK, typename T, bool ADJ = false>
 __global__ void __launch_bounds__(kThreads, 3) k2_synthesize(const K2Args a) {
     constexpr int NH = 32 / HR;             // frames overlapping one hop (win / hop)
     B200_DYN_SMEM(float, smem);
@@ -906,12 +962,14 @@ __global__ void __launch_bounds__(kThreads, 3) k2_synthesize(const K2Args a) {
         if (jp_hi <= g.pad) continue;
         const long long jlo = g.pad + kN / 2, jhi = jp_hi + kN / 2;
         const int h_lo = (int)(jlo / H), h_hi = (int)((jhi + H - 1) / H);
-        const int hs = h_lo + run * a.run;
-        const int he = min(hs + a.run, h_hi);
+        // the adjoint runs the frames [f_lo, f_hi] that touch the centre and writes every hop they overlap
+        const int f_lo = ADJ ? max(0, h_lo - (NH - 1)) : 0, f_hi = ADJ ? min(h_hi - 1, g.T - 1) : g.T - 1;
+        const int hs = (ADJ ? f_lo : h_lo) + run * a.run;
+        const int he = min(hs + a.run, ADJ ? f_hi + NH : h_hi);
         if (hs >= he) continue;
-        int t_start = max(0, hs - (NH - 1));
+        int t_start = max(f_lo, hs - (NH - 1));
         if (a.zcache) t_start &= ~1;                 // k1 packed frames (2j, 2j+1): walk the same pairs
-        const int t_last = min(he - 1, g.T - 1);
+        const int t_last = min(he - 1, f_hi);
         const T* xrow = static_cast<const T*>(a.x) + (long long)c * g.in_stride;
         T* yrow = static_cast<T*>(a.y) + (long long)c * g.out_stride;
         const unsigned short* mrow = FMASK ? nullptr : a.num + (long long)ul * num_unit_stride(g.T);
@@ -935,7 +993,9 @@ __global__ void __launch_bounds__(kThreads, 3) k2_synthesize(const K2Args a) {
             if (va) {                                   // vb implies va
                 const long long base = (long long)t * H - kN / 2;
                 float re[32], im[32];
-                if (!a.zcache) load_frame_pair<HR>(re, im, xrow, base, i1, g.Lp, g.n_total, s_wa, lane, vb);
+                if (ADJ) load_adjoint_pair<HR>(re, im, xrow, t, base, i1, g.pad, jp_hi, H, g.T, s_invn, s_ws,
+                                               a.tb.ws_to_w, s_wa, lane, vb);
+                else if (!a.zcache) load_frame_pair<HR>(re, im, xrow, base, i1, g.Lp, g.n_total, s_wa, lane, vb);
                 const long long offA = (long long)t * kFPad, offB = (long long)(vb ? t + 1 : t) * kFPad;
                 // the masks of this pair are requested now, a whole FFT before the apply step needs them
                 float mka[kFW], mkb[FMASK ? kFW : 1];         // uint16 numerators travel packed two per register
@@ -1050,7 +1110,15 @@ __global__ void __launch_bounds__(kThreads, 3) k2_synthesize(const K2Args a) {
                 }
             }
             // hops t and t+1 are now complete (all frames <= t+1 have been added)
-            {
+            if (ADJ) {                                       // un-normalised, the whole padded span
+                float* arow = a.adj + (long long)ul * a.adj_pitch;
+#pragma unroll
+                for (int r = 0; r < 2 * HR; ++r) {
+                    const int hop = t + r / HR;
+                    const long long jp = (long long)t * H - kN / 2 + 32 * r + lane;
+                    if (hop >= hs && hop < he && jp >= 0 && jp < g.Lp) arow[jp] = acc[r];
+                }
+            } else {
                 const long long jp0 = (long long)t * H - kN / 2;             // chunk-local index of row 0, lane 0
                 if (t >= hs && t + 1 < he && t >= NH - 1 && t + 1 <= g.T - 1 && jp0 >= g.pad &&
                     jp0 + 2 * H <= jp_hi) {

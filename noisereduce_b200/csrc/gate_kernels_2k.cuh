@@ -157,10 +157,56 @@ struct K22Args {
     const float* fmask;        // [n_units][T][FPad2] final multiplicative masks
     int run, n_runs;           // output hops per work item
     DebugTap dbg;              // mask: [T][F2]
+    // k2_synthesize_2k<true>: the adjoint of a unit (b200gate_adjoint), as k2_synthesize<.., ADJ>: x is the gradient g,
+    // read on the unit's centre only and divided by the overlap-add norm; the un-normalised overlap-add of the padded
+    // span goes to adj[ul][0, Lp)
+    float* adj;
+    long long adj_pitch;
 };
+
+// 1 / (sum of w^2 over the frames overlapping sample `ro` of hop `hop`), as k2_synthesize_2k's edge hops compute it
+__device__ B200_NOINLINE float inv_norm_2k(int hop, int ro, int H, int T, const float2* __restrict__ s_ws2,
+                                             float ws_to_w) {
+    float nrm = 0.f;
+    for (int i = 0; i < 4; ++i) {
+        const int tf = hop - i;
+        if (tf >= 0 && tf <= T - 1) {
+            const int n = i * H + ro;
+            const float2 wp = s_ws2[n >> 1];
+            const float w = ((n & 1) ? wp.y : wp.x) * ws_to_w;
+            nrm = fmaf(w, w, nrm);
+        }
+    }
+    return nrm > 1e-10f ? 1.0f / nrm : 1.0f;
+}
+
+// the adjoint's input frame t: g / norm on the centre [pad, jp_hi), zero elsewhere, windowed (pairs as load_frame_2k).
+// Sample 2 (lane + 32 r) + par of the frame is sample (r % 8) * 64 + 2 lane + par of hop t + r / 8.
+__device__ __forceinline__ void load_adjoint_2k(float (&re)[32], float (&im)[32], const float* __restrict__ grow, int t,
+                                                long long base, long long i1, long long pad, long long jp_hi, int H, int T,
+                                                const float2* __restrict__ s_invn2, const float2* __restrict__ s_ws2,
+                                                float ws_to_w, const float2* __restrict__ s_wa2, int lane) {
+    const bool interior = t >= 3 && t + 3 <= T - 1;          // every hop of the frame has the interior norm
+#pragma unroll
+    for (int r = 0; r < 32; ++r) {
+        const long long j = base + 2 * (lane + 32 * r);
+        const float2 w = s_wa2[lane + 32 * r];
+        float2 inv;
+        if (interior) {
+            inv = s_invn2[(r & 7) * 32 + lane];
+        } else {
+            const int ro = (r & 7) * 64 + 2 * lane;
+            inv = make_float2(inv_norm_2k(t + (r >> 3), ro, H, T, s_ws2, ws_to_w),
+                              inv_norm_2k(t + (r >> 3), ro + 1, H, T, s_ws2, ws_to_w));
+        }
+        re[r] = (j >= pad && j < jp_hi) ? __ldg(grow + i1 + j) * inv.x * w.x : 0.0f;
+        im[r] = (j + 1 >= pad && j + 1 < jp_hi) ? __ldg(grow + i1 + j + 1) * inv.y * w.y : 0.0f;
+    }
+}
 
 constexpr int k22_smem_floats() { return k2k_table_floats() + 2 * 1024 + 2 * 256 + kWarps * kExchFloats; }
 
+template <bool ADJ = false>
 __global__ void __launch_bounds__(kThreads, 2) k2_synthesize_2k(const K22Args a) {
     constexpr int HR = 8, NH = 4;
     B200_DYN_SMEM(float, smem);
@@ -201,11 +247,13 @@ __global__ void __launch_bounds__(kThreads, 2) k2_synthesize_2k(const K22Args a)
         if (jp_hi <= g.pad) continue;
         const long long jlo = g.pad + kN2 / 2, jhi = jp_hi + kN2 / 2;
         const int h_lo = (int)(jlo / H), h_hi = (int)((jhi + H - 1) / H);
-        const int hs = h_lo + run * a.run;
-        const int he = min(hs + a.run, h_hi);
+        // the adjoint runs the frames [f_lo, f_hi] that touch the centre and writes every hop they overlap
+        const int f_lo = ADJ ? max(0, h_lo - (NH - 1)) : 0, f_hi = ADJ ? min(h_hi - 1, g.T - 1) : g.T - 1;
+        const int hs = (ADJ ? f_lo : h_lo) + run * a.run;
+        const int he = min(hs + a.run, ADJ ? f_hi + NH : h_hi);
         if (hs >= he) continue;
-        const int t_start = max(0, hs - (NH - 1));
-        const int t_last = min(he - 1, g.T - 1);
+        const int t_start = max(f_lo, hs - (NH - 1));
+        const int t_last = min(he - 1, f_hi);
         const float* xrow = a.x + (long long)c * g.in_stride;
         float* yrow = a.y + (long long)c * g.out_stride;
         const float* frow = a.fmask + (long long)ul * g.T * kFPad2;
@@ -218,7 +266,9 @@ __global__ void __launch_bounds__(kThreads, 2) k2_synthesize_2k(const K22Args a)
             if (t <= t_last) {
                 const long long base = (long long)t * H - kN2 / 2;
                 float re[32], im[32];
-                load_frame_2k(re, im, xrow, base, i1, g.Lp, g.n_total, s_wa2, lane);
+                if (ADJ) load_adjoint_2k(re, im, xrow, t, base, i1, g.pad, jp_hi, H, g.T, s_invn2, s_ws2, a.tb.ws_to_w,
+                                         s_wa2, lane);
+                else load_frame_2k(re, im, xrow, base, i1, g.Lp, g.n_total, s_wa2, lane);
                 const float* mrow = frow + (long long)t * kFPad2;
                 if (a.dbg.ul == ul) {
 #pragma unroll 1
@@ -295,7 +345,18 @@ __global__ void __launch_bounds__(kThreads, 2) k2_synthesize_2k(const K22Args a)
                 }
             }
             // hop t is complete: rows 0..7 (pairs) = samples [t*512, (t+1)*512)
-            if (t >= hs) {
+            if (ADJ) {                                       // un-normalised, the whole padded span
+                if (t >= hs) {
+                    float* arow = a.adj + (long long)ul * a.adj_pitch;
+                    const long long jp0 = (long long)t * H - kN2 / 2;
+#pragma unroll
+                    for (int r = 0; r < HR; ++r) {
+                        const long long jp = jp0 + 64 * r + 2 * lane;
+                        if (jp >= 0 && jp < g.Lp) arow[jp] = acc_e[r];
+                        if (jp + 1 >= 0 && jp + 1 < g.Lp) arow[jp + 1] = acc_o[r];
+                    }
+                }
+            } else if (t >= hs) {
                 const long long jp0 = (long long)t * H - kN2 / 2;          // chunk-local index of row 0, pair 0
                 float* d0 = yrow + i1 + jp0 + 2 * lane;
                 if (t >= NH - 1 && t <= g.T - 1 && jp0 >= g.pad && jp0 + H <= jp_hi &&

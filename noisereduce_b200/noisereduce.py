@@ -46,6 +46,8 @@ def reduce_noise(
     integer and bool tensors are promoted to float64 and cast back on the device with numpy's rules; bfloat16 raises
     TypeError.  CPU tensors take the numpy route and return numpy arrays, as before.  See spectralgate/base.py.  With
     use_torch=True and a CUDA y, ``device`` left at "cuda" means y's device; another device raises ValueError.
+    A CUDA y that requires grad (use_torch=False) gives a differentiable result with TorchGate's gradient convention
+    (masks held constant); the call then returns without waiting for the device (spectralgate/base.py, _gate_function).
     """
     if use_torch:
         if n_jobs != 1:                                         # noisereduce.py:115-118

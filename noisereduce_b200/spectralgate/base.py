@@ -137,6 +137,11 @@ class SpectralGate:
     reduce_noise() builds the object, calls get_traces() and drops the object, so it returns only once the device is
     idle, including work on other streams.  A caller who wants the result still in flight keeps the object and calls
     get_traces().
+
+    A CUDA ``y`` that requires grad (with grad mode on) makes the result differentiable (`_gate_function`): the graph
+    then holds this object, so reduce_noise() returns without destroying the handle and without waiting for the device.
+    The handle's device workspace (allocated by the library, outside torch's allocator) is held with it until the graph
+    is freed.
     """
 
     def __init__(
@@ -324,15 +329,21 @@ class SpectralGate:
             if start_frame < 0 or end_frame > self.n_frames:
                 raise ValueError("start_frame / end_frame outside the recording")
             first, last = int(start_frame / self._chunk_size), int((end_frame - 1) / self._chunk_size)
-            self._gate.set_range(1, first, last)
+            rng = (1, first, last)
             lo = start_frame
             span = (first * self._chunk_size, min(self.n_frames, (last + 1) * self._chunk_size))
         else:
             if not 0 < end_frame <= self.n_frames:
                 raise ValueError("end_frame outside the recording")
-            self._gate.set_range(2, int(end_frame))
+            rng = (2, int(end_frame))
             lo = 0
             span = (0, int(end_frame))
+        # (the torch route, reduce_noise(use_torch=True), detaches as the reference's does)
+        if (self._site is not None and self._site.torch.is_grad_enabled() and self.y.requires_grad
+                and self._gate.params.surface == _cabi.SURFACE_NUMPY):
+            res = _gate_function().apply(self.y, self, rng, lo, end_frame, span)
+            return res.flatten() if self.flat else res
+        self._gate.set_range(*rng)
         try:
             if self._site is None:
                 res = self._run(self.y, lo, end_frame)
@@ -346,3 +357,75 @@ class SpectralGate:
     def _on_device(self):
         """Context of the handle calls: the samples' CUDA device on the device route, nothing otherwise."""
         return contextlib.nullcontext() if self._site is None else self._site.active()
+
+
+# ---- backpropagation on the device route ------------------------------------------------------------------------------
+_GATE_FUNCTION = None
+
+
+def _gate_function():
+    """The torch.autograd.Function get_traces() runs through when the samples are a CUDA tensor that requires grad (and
+    grad mode is on).  Built on first use, so that torch is only imported by callers that pass tensors.
+
+    The gradient is TorchGate's convention (torchgate.py:223-262): the thresholds, the mask decisions, the top_db row
+    flags and the non-stationary noise floor are constants, and the gradient flows through STFT -> mask -> iSTFT and the
+    chunk assembly.  For the stationary gate the decisions are piecewise constant in y (thresholds taken from y's own
+    first chunk included), so this is the true derivative everywhere except where a decision sits exactly on its
+    threshold.  For the non-stationary gate the noise floor's dependence on y is dropped, as TorchGate drops its moving
+    mean.  y_noise gets no gradient.
+
+    The forward keeps every unit's final masks in a store allocated with torch on y's device (b200gate_set_mask_store);
+    the backward applies the gate's adjoint with them (b200gate_adjoint) on the current stream.  The saved context holds
+    the gate object, so its library handle lives until the graph is freed: in this mode reduce_noise() returns without
+    waiting for the device.  float16 samples are promoted to float64 and cast back as in the forward; the gradient passes
+    those casts as it passes Tensor.to.  Double backward raises."""
+    global _GATE_FUNCTION
+    if _GATE_FUNCTION is not None:
+        return _GATE_FUNCTION
+    torch = sys.modules["torch"]
+    from torch.autograd.function import once_differentiable
+
+    class GateFunction(torch.autograd.Function):
+        @staticmethod
+        def forward(ctx, y2d, sg, rng, lo, hi, span):
+            site = sg._site
+            gate = sg._gate
+            C, N = y2d.shape
+            with site.active():
+                gate.set_range(*rng)
+                try:
+                    nbytes = gate.mask_store_bytes(C, N)
+                    store = torch.empty(nbytes, dtype=torch.uint8, device=site.device)
+                    gate.set_mask_store(store.data_ptr(), nbytes)
+                    try:
+                        res = sg._run_device(lo, hi, *span)
+                    finally:
+                        gate.set_mask_store(None)
+                finally:
+                    gate.set_range(0)
+            ctx.sg, ctx.store, ctx.rng, ctx.lo, ctx.hi, ctx.span = sg, store, rng, lo, hi, span
+            ctx.y_dtype = y2d.dtype
+            return res
+
+        @staticmethod
+        @once_differentiable
+        def backward(ctx, g):
+            sg, site = ctx.sg, ctx.sg._site
+            C, N = sg.n_channels, sg.n_frames
+            lo, hi, (w_lo, w_hi) = ctx.lo, ctx.hi, ctx.span
+            gdt = np.dtype(np.float32) if sg._dtype == np.float32 else np.dtype(np.float64)   # the kernels' dtype
+            tdt = torch.from_numpy(np.empty(0, gdt)).dtype
+            with site.active():
+                gs = torch.zeros((C, w_hi - w_lo), dtype=tdt, device=site.device)
+                gs[:, lo - w_lo: hi - w_lo] = g.reshape(C, hi - lo).to(tdt)
+                grad = torch.empty((C, N), dtype=tdt, device=site.device)
+                sg._gate.set_range(*ctx.rng)
+                try:
+                    sg._gate.adjoint_device(ctx.store.data_ptr(), gs.data_ptr() - w_lo * gdt.itemsize, grad.data_ptr(),
+                                            gdt, C, N, w_hi - w_lo, N, site.stream)
+                finally:
+                    sg._gate.set_range(0)
+            return grad.to(ctx.y_dtype), None, None, None, None, None
+
+    _GATE_FUNCTION = GateFunction
+    return GateFunction
