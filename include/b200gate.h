@@ -174,6 +174,31 @@ int b200gate_torch_apply_masks(b200gate_handle* h, const void* in, void* out, in
 int b200gate_run(b200gate_handle* h, const void* in, void* out, int dtype, int64_t C, int64_t N,
                  int64_t in_stride, int64_t out_stride, int is_device, void* cuda_stream);
 
+/* Rows of different lengths in one call (numpy surface): every row is a recording of its own, one channel of `n`
+ * samples, and out[0, n) of row r holds exactly what b200gate_run writes for that channel of its [channels][n] recording -- the chunk
+ * grid, the padded span, the frame count and everything derived from them (smoothing edges, overlap-add edge norm,
+ * top_db row maxima, the non-stationary follower's sweeps and its choice between regenerating and storing the forward
+ * sweep) are taken per row.  The channels of a multi-channel recording are simply consecutive rows: with the thresholds
+ * fixed (b200gate_noise_stats / b200gate_set_noise_threshold, once for all rows) a channel's result depends on no other
+ * channel in either gate.  The units of all rows share the workspace at the pitch of the call's longest unit.
+ * Device pointers (is_device = 1) are read and written where they are and the call only enqueues on cuda_stream, without
+ * waiting for the device.  Host rows must lie in one buffer each way: they travel as the span that covers them, one copy
+ * in and one copy out (bytes of the output span between rows are overwritten), and the call returns with the result in
+ * place.  b200gate_get_stats counts the units of all rows and their own frames.
+ * B200GATE_ERR_STATE: a torch surface, an open stream, a mask store set, a range mode other than 0, a stationary gate
+ * without thresholds.  B200GATE_ERR_ARG: a geometry other than n_fft = win_length = 1024, hop_length = 256; non-zero
+ * path_flags; smoothing extents beyond the in-synthesis smoothing (stationary: n_grad_time > 13 or n_grad_freq > 17) or
+ * beyond the streaming float-mask smoothing; n <= 0, channels <= 0, a null pointer, out overlapping in; scattered host rows.  A refused
+ * call changes nothing on the handle. */
+typedef struct b200gate_row {
+    const void* in; void* out; int64_t n;
+    int64_t channels;   /* rows of the recording this row is a channel of (>= 1).  Sizes the synthesis work items as
+                         * b200gate_run does for a [channels][n] recording that fits one workspace batch: the last bit
+                         * of the hops at work-item seams depends on that length, everything else does not */
+} b200gate_row;
+int b200gate_run_rows(b200gate_handle* h, const b200gate_row* rows, int64_t n_rows, int dtype, int is_device,
+                      void* cuda_stream);
+
 /* Sub-range processing for the next b200gate_run calls (SpectralGate.get_traces(start_frame, end_frame),
  * base.py:167-226).  mode 0: the whole recording (default).  mode 1: only chunks [a, b] of the chunk grid
  * anchored at sample 0 (the reference's chunked branch); samples outside those chunks are not written.

@@ -37,7 +37,7 @@ EXPORTS = [
     "b200gate_run_sharded", "b200gate_peer_push", "b200gate_peer_barrier", "b200gate_torch_apply_masks",
     "b200gate_host_alloc", "b200gate_host_free",
     "b200gate_stream_begin", "b200gate_stream_push", "b200gate_stream_finish", "b200gate_convert",
-    "b200gate_mask_store_bytes", "b200gate_set_mask_store", "b200gate_adjoint",
+    "b200gate_mask_store_bytes", "b200gate_set_mask_store", "b200gate_adjoint", "b200gate_run_rows",
 ]
 
 
@@ -67,6 +67,11 @@ class Stats(C.Structure):
 
     def as_dict(self):
         return {k: getattr(self, k) for k, _ in self._fields_}
+
+
+class Row(C.Structure):
+    """b200gate_row: one channel of one recording (b200gate_run_rows)."""
+    _fields_ = [("in_", C.c_void_p), ("out", C.c_void_p), ("n", C.c_int64), ("channels", C.c_int64)]
 
 
 class GateError(RuntimeError):
@@ -131,6 +136,7 @@ class GateLibrary:
         d.b200gate_mask_store_bytes.argtypes = [vp, i64, i64, C.POINTER(i64)]
         d.b200gate_set_mask_store.argtypes = [vp, vp, i64]
         d.b200gate_adjoint.argtypes = [vp, vp, vp, vp, C.c_int, i64, i64, i64, i64, C.c_int, vp]
+        d.b200gate_run_rows.argtypes = [vp, C.POINTER(Row), i64, C.c_int, C.c_int, vp]
 
 
 def format_code(dt) -> int:
@@ -320,6 +326,11 @@ class Gate:
     def run_device(self, in_ptr, out_ptr, dtype, C_, N, in_stride, out_stride, stream=None):
         self._check(self.lib.dll.b200gate_run(
             self._h, in_ptr, out_ptr, dtype_code(dtype), C_, N, in_stride, out_stride, 1, stream))
+
+    def run_rows(self, rows, dtype, is_device, stream=None):
+        """b200gate_run_rows on (in_ptr, out_ptr, n, channels of the recording) tuples: one recording channel each (include/b200gate.h)."""
+        arr = (Row * len(rows))(*rows)
+        self._check(self.lib.dll.b200gate_run_rows(self._h, arr, len(rows), dtype_code(dtype), 1 if is_device else 0, stream))
 
     def run_sharded(self, in_ptr, dtype, C_local, N, in_stride, gathered_local, gathered_peers, flags_local, flags_peers,
                     epoch, rank, world, groups, push_ctas, compute_stream, comm_stream):

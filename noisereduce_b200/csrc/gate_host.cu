@@ -118,6 +118,13 @@ struct b200gate_handle {
     long long s_cap = 0, s_slice = 0, s_ocap = 0;  // window pitch, samples one slice appends at most, output pitch
     void *d_swin = nullptr, *d_sout = nullptr;
     size_t swin_bytes = 0, sout_bytes = 0;
+    // b200gate_run_rows: the call's unit table, written by the host into hp_units and copied to d_units on the call's
+    // stream; ev_units marks that copy, so the next call can rewrite hp_units without waiting for the device
+    UnitDesc* hp_units = nullptr;
+    size_t hp_units_bytes = 0;
+    void* d_units = nullptr;
+    size_t units_bytes = 0;
+    cudaEvent_t ev_units = nullptr;
     // debug taps
     long long dbg_chunk = -1, dbg_channel = -1;
     long long dbg_T = 0;
@@ -739,9 +746,10 @@ static void launch_stationary_numerators(const b200gate_handle* h, const SmoothA
 
 // Float-mask smoothing (non-stationary gate, TorchGate moving-mean gate): the box form for 1 <= nf <= 12 (k_smooth_box,
 // compiled per nf), else the tap-loop streaming kernel, else (ring too large for shared memory) the tile kernel.
-#define B200_SMOOTH_BOX_CASE(NF_) case NF_: { auto kern_ = k_smooth_box<NF_>; \
+#define B200_SMOOTH_BOX_CASE(NF_) case NF_: { auto kern_ = ROWS ? k_smooth_box<NF_, true> : k_smooth_box<NF_>; \
         if (set_attr) cudaFuncSetAttribute(kern_, cudaFuncAttributeMaxDynamicSharedMemorySize, 200 * 1024); \
         else B200_LAUNCH(kern_, grid, dim3(sa.FPad / 4), smem, st, sa); } break;
+template <bool ROWS = false>
 static void smooth_box_dispatch(const SmoothFArgs& sa, int nf, dim3 grid, size_t smem, cudaStream_t st, bool set_attr) {
     switch (nf) {
         B200_SMOOTH_BOX_CASE(1) B200_SMOOTH_BOX_CASE(2) B200_SMOOTH_BOX_CASE(3) B200_SMOOTH_BOX_CASE(4)
@@ -750,21 +758,27 @@ static void smooth_box_dispatch(const SmoothFArgs& sa, int nf, dim3 grid, size_t
         default: break;
     }
 }
-static void launch_smooth_float(SmoothFArgs sa, int nf, int nt, int tf_lo, int tf_hi, int nu, int path_flags, cudaStream_t st) {
+// ROWS (b200gate_run_rows; sa.units set, tf_hi the largest of the batch): the two streaming kernels only -- false when the
+// ring does not fit shared memory.
+template <bool ROWS = false>
+static bool launch_smooth_float(SmoothFArgs sa, int nf, int nt, int tf_lo, int tf_hi, int nu, int path_flags, cudaStream_t st) {
     const bool box_ok = nf >= 1 && nf <= 12 && sa.FPad - sa.F >= 12 && smoothb_smem_bytes(sa.FPad, nt) <= 200 * 1024 &&
                         !(path_flags & 32) && !(path_flags & 128);
     if (box_ok) {
         sa.TT = 256;                        // frames per strip (2 nt warm-up rows each)
         const int strips = (tf_hi - tf_lo + sa.TT - 1) / sa.TT;
-        smooth_box_dispatch(sa, nf, dim3(strips, nu), smoothb_smem_bytes(sa.FPad, nt), st, false);
+        smooth_box_dispatch<ROWS>(sa, nf, dim3(strips, nu), smoothb_smem_bytes(sa.FPad, nt), st, false);
     } else if (smooths_smem_bytes(sa.FPad, nf, nt) <= 200 * 1024 && !(path_flags & 32)) {
         sa.TT = 256;
         const int strips = (tf_hi - tf_lo + sa.TT - 1) / sa.TT;
-        B200_LAUNCH(k_smooth_stream, dim3(strips, nu), dim3(sa.FPad / 4), smooths_smem_bytes(sa.FPad, nf, nt), st, sa);
+        B200_LAUNCH(k_smooth_stream<ROWS>, dim3(strips, nu), dim3(sa.FPad / 4), smooths_smem_bytes(sa.FPad, nf, nt), st, sa);
+    } else if (ROWS) {
+        return false;
     } else {
         const int tiles = (tf_hi - tf_lo + sa.TT - 1) / sa.TT;
         B200_LAUNCH(k_smooth_f, dim3(tiles, nu), dim3(256), smoothf_smem_bytes(sa.TT, sa.FPad, nf), st, sa);
     }
+    return true;
 }
 
 // k_iir_sigmoid may rebuild its forward sweep by the inverse recurrence (IirArgs::regen) only where the bound on the
@@ -987,8 +1001,20 @@ int b200gate_create(const b200gate_params* p, b200gate_handle** out) {
                 cudaFuncSetAttribute(k2c_synthesize<8, kMaskBitsBlend, T>, cudaFuncAttributeMaxDynamicSharedMemorySize, k2c_smem_bytes<kMaskBitsBlend>());
             });
         cudaFuncSetAttribute(k_smooth_f, cudaFuncAttributeMaxDynamicSharedMemorySize, 200 * 1024);
-        cudaFuncSetAttribute(k_smooth_stream, cudaFuncAttributeMaxDynamicSharedMemorySize, 200 * 1024);
+        cudaFuncSetAttribute(k_smooth_stream<>, cudaFuncAttributeMaxDynamicSharedMemorySize, 200 * 1024);
         for (int nfb = 1; nfb <= 12; ++nfb) smooth_box_dispatch(SmoothFArgs{}, nfb, dim3(1), 0, nullptr, true);
+        // b200gate_run_rows: the ROWS instantiations of the default kernel selection
+        for (int dt = 0; dt < 3; ++dt)
+            B200_WITH_DTYPE(dt, {
+                cudaFuncSetAttribute(k1_analyze<8, T, false, true>, cudaFuncAttributeMaxDynamicSharedMemorySize, k1_smem_floats() * 4);
+                cudaFuncSetAttribute(k1_analyze<8, T, true, true>, cudaFuncAttributeMaxDynamicSharedMemorySize, k1_smem_floats() * 4);
+                cudaFuncSetAttribute(k1n_magnitude<8, T, true>, cudaFuncAttributeMaxDynamicSharedMemorySize, k1n_smem_floats() * 4);
+                cudaFuncSetAttribute(k2c_synthesize<8, kMaskF32, T, true>, cudaFuncAttributeMaxDynamicSharedMemorySize, k2c_smem_bytes<kMaskF32>());
+                cudaFuncSetAttribute(k2c_synthesize<8, kMaskBits, T, true>, cudaFuncAttributeMaxDynamicSharedMemorySize, k2c_smem_bytes<kMaskBits>());
+                cudaFuncSetAttribute(k2c_synthesize<8, kMaskBitsBlend, T, true>, cudaFuncAttributeMaxDynamicSharedMemorySize, k2c_smem_bytes<kMaskBitsBlend>());
+            });
+        cudaFuncSetAttribute(k_smooth_stream<true>, cudaFuncAttributeMaxDynamicSharedMemorySize, 200 * 1024);
+        for (int nfb = 1; nfb <= 12; ++nfb) smooth_box_dispatch<true>(SmoothFArgs{}, nfb, dim3(1), 0, nullptr, true);
         cudaFuncSetAttribute(k1n_magnitude_2k, cudaFuncAttributeMaxDynamicSharedMemorySize, k1n2_smem_floats() * 4);
         cudaFuncSetAttribute(k2_synthesize_2k<>, cudaFuncAttributeMaxDynamicSharedMemorySize, k22_smem_floats() * 4);
         cudaFuncSetAttribute(k2_synthesize_2k<true>, cudaFuncAttributeMaxDynamicSharedMemorySize, k22_smem_floats() * 4);
@@ -1039,6 +1065,9 @@ void b200gate_destroy(b200gate_handle* h) {
     if (h->h_cnt) cudaFreeHost(h->h_cnt);
     for (int i = 0; i < 2; ++i) { g_pinned_pool.give(h->hp_in[i], h->hp_in_bytes[i]); g_pinned_pool.give(h->hp_out[i], h->hp_out_bytes[i]); }
     if (h->d_need_rowmax) cudaFree(h->d_need_rowmax);
+    g_pinned_pool.give(h->hp_units, h->hp_units_bytes);
+    if (h->d_units) cudaFree(h->d_units);
+    if (h->ev_units) cudaEventDestroy(h->ev_units);
     for (cudaEvent_t e : h->stage_ev) cudaEventDestroy(e);
     for (cudaEvent_t e : h->pipe_ev) cudaEventDestroy(e);
     if (h->s_h2d) cudaStreamDestroy(h->s_h2d);
@@ -2336,6 +2365,296 @@ int b200gate_run(b200gate_handle* h, const void* in, void* out, int dtype, int64
     const int rc = run_core(h, in, out, dtype, C, N, in_stride, out_stride, is_device, stream, 0);
     if (h) h->keep_masks = false;
     return rc;
+}
+
+// ---- b200gate_run_rows: rows of different lengths in one call ---------------------------------------------------------
+// Every row is a recording of its own: it is cut into units exactly as run_grid() cuts a [1][n] recording (one padded
+// chunk of n + 2 pad samples when n <= chunk_size, else chunks of chunk_size + 2 pad), the units of all rows form one
+// table (UnitDesc) and the ROWS instantiations of the default kernels of run_core walk it.  Per-unit buffers have the
+// pitch of the call's longest unit; everything that run_core derives from T or Lp is derived per unit here.
+int b200gate_run_rows(b200gate_handle* h, const b200gate_row* rows, int64_t n_rows, int dtype, int is_device, void* stream) {
+    if (!h || !rows || n_rows <= 0 || dtype_size(dtype) == 0) return fail(h, B200GATE_ERR_ARG, "bad argument");
+    if (h->s_open) return fail(h, B200GATE_ERR_STATE, "a stream is open on this handle (b200gate_stream_finish first)");
+    const b200gate_params& p = h->p;
+    if (p.surface != B200GATE_SURFACE_NUMPY) return fail(h, B200GATE_ERR_STATE, "b200gate_run_rows is for the numpy surface");
+    if (h->mask_store) return fail(h, B200GATE_ERR_STATE, "b200gate_run_rows keeps no masks (b200gate_set_mask_store(NULL) first)");
+    if (h->range_mode != 0) return fail(h, B200GATE_ERR_STATE, "b200gate_run_rows runs whole rows (b200gate_set_range(0) first)");
+    if (h->generic || p.n_fft != kN) return fail(h, B200GATE_ERR_ARG, "b200gate_run_rows needs n_fft = win_length = 1024, hop_length = 256");
+    if (p.path_flags != 0) return fail(h, B200GATE_ERR_ARG, "b200gate_run_rows runs the default kernel selection (path_flags = 0)");
+    const bool stat = p.stationary != 0;
+    const int nf = p.n_grad_freq, nt = p.n_grad_time;
+    if (stat && !packed_smoothing_fits(nf, nt))
+        return fail(h, B200GATE_ERR_ARG, "b200gate_run_rows: stationary smoothing extents (%d, %d) beyond the in-synthesis smoothing", nf, nt);
+    if (!stat && !((nf >= 1 && nf <= 12 && smoothb_smem_bytes(kFPad, nt) <= 200 * 1024) || smooths_smem_bytes(kFPad, nf, nt) <= 200 * 1024))
+        return fail(h, B200GATE_ERR_ARG, "b200gate_run_rows: smoothing extents (%d, %d) beyond the streaming smoothing kernels", nf, nt);
+    if (stat && !h->have_thresh) return fail(h, B200GATE_ERR_STATE, "stationary gate: call b200gate_noise_stats first");
+    cudaStream_t st = (cudaStream_t)stream;
+    const size_t es = dtype_size(dtype);
+    const int H = p.hop_length;
+    const long long pad = p.padding, cs = p.chunk_size;
+
+    // ---- the unit table -------------------------------------------------------------------------------------
+    const char *in_lo = nullptr, *in_hi = nullptr, *out_lo = nullptr, *out_hi = nullptr;    // spans covering the rows
+    size_t row_bytes = 0;
+    long long U = 0;
+    for (int64_t r = 0; r < n_rows; ++r) {
+        const b200gate_row& rw = rows[r];
+        if (!rw.in || !rw.out || rw.n <= 0 || rw.channels <= 0)
+            return fail(h, B200GATE_ERR_ARG, "row %lld: null pointer, no samples or no channels", (long long)r);
+        const char *a = (const char*)rw.in, *b = (const char*)rw.out;
+        const size_t nb = (size_t)rw.n * es;
+        if (a < b + nb && b < a + nb) return fail(h, B200GATE_ERR_ARG, "row %lld: out aliases in", (long long)r);
+        const long long Lp = (cs > 0 && rw.n > cs ? cs : rw.n) + 2 * pad;
+        if (Lp / H > 0x3fffffffLL) return fail(h, B200GATE_ERR_ARG, "problem too large");
+        U += cs > 0 && rw.n > cs ? (rw.n - 1) / cs + 1 : 1;
+        if (!in_lo || a < in_lo) in_lo = a;
+        if (!in_hi || a + nb > in_hi) in_hi = a + nb;
+        if (!out_lo || b < out_lo) out_lo = b;
+        if (!out_hi || b + nb > out_hi) out_hi = b + nb;
+        row_bytes += nb;
+    }
+    if (U > 0x7fffffffLL) return fail(h, B200GATE_ERR_ARG, "problem too large");
+    // host rows travel as the two spans that cover them, one copy each way: they must come packed in one buffer
+    const size_t in_span = (size_t)(in_hi - in_lo), out_span = (size_t)(out_hi - out_lo);
+    if (!is_device && std::max(in_span, out_span) > 2 * row_bytes + 4096 * (size_t)n_rows)
+        return fail(h, B200GATE_ERR_ARG, "host rows must lie in one buffer (they are copied as the span that covers them)");
+    const size_t tbytes = (size_t)U * sizeof(UnitDesc);
+    if (!h->ev_units) CK(h, cudaEventCreateWithFlags(&h->ev_units, cudaEventDisableTiming));
+    else CK(h, cudaEventSynchronize(h->ev_units));             // the last call's table has left hp_units
+    if (h->hp_units_bytes < tbytes) {
+        g_pinned_pool.give(h->hp_units, h->hp_units_bytes);
+        h->hp_units = (UnitDesc*)g_pinned_pool.take(tbytes, &h->hp_units_bytes);
+        if (!h->hp_units) { h->hp_units_bytes = 0; return fail(h, B200GATE_ERR_NOMEM, "pinned unit table (%zu bytes)", tbytes); }
+    }
+    {
+        int rc;
+        if ((rc = ensure(h, &h->d_units, &h->units_bytes, tbytes))) return rc;
+        if (!is_device) {
+            if ((rc = ensure(h, (void**)&h->d_in, &h->in_bytes, in_span))) return rc;
+            if ((rc = ensure(h, (void**)&h->d_out, &h->out_bytes, out_span))) return rc;
+        }
+    }
+    double b_iir = 0.0;
+    if (!stat) {
+        const double tfr = p.time_constant_s * p.sr / (double)H;                    // nonstationary.py:109-114
+        b_iir = (sqrt(1.0 + 4.0 * tfr * tfr) - 1.0) / (2.0 * tfr * tfr);
+    }
+    // frames whose masks the synthesis needs: [tf_lo, tf_hi) with the first one shared by every unit (run_core)
+    const int h_lo = (int)((pad + kN / 2) / H);
+    const int tf_lo = std::max(0, h_lo - 3) & ~1;
+    int T_max = 0, tf_hi_max = 0;
+    long long n_runs2 = 0;                                      // synthesis work items per unit: the most any unit needs
+    const int resident = h->num_sm * 3;
+    long long frames = 0;
+    std::vector<long long> zero_units;                          // units whose centre reaches past their istft output
+    {
+        long long u = 0;
+        for (int64_t r = 0; r < n_rows; ++r) {
+            const b200gate_row& rw = rows[r];
+            const bool chunked = cs > 0 && rw.n > cs;
+            const long long step = chunked ? cs : rw.n, nch = chunked ? (rw.n - 1) / cs + 1 : 1;
+            const void* x = is_device ? rw.in : (const void*)((const char*)h->d_in + ((const char*)rw.in - in_lo));
+            void* y = is_device ? rw.out : (void*)((char*)h->d_out + ((const char*)rw.out - out_lo));
+            for (long long ic = 0; ic < nch; ++ic, ++u) {
+                UnitDesc& d = h->hp_units[u];
+                d.x = x; d.y = y; d.n_total = rw.n;
+                d.i1 = ic * step - pad;
+                d.Lp = step + 2 * pad;
+                d.o_lo = ic * step;
+                d.o_hi = std::min<long long>(rw.n, (ic + 1) * step);
+                d.T = (int)(d.Lp / H) + 1;
+                const long long sig_len = (long long)(d.T - 1) * H;
+                const long long jp_hi = std::min(pad + step, sig_len);
+                int h_hi = 0;
+                d.tf_hi = 0;
+                if (jp_hi > pad) {
+                    h_hi = (int)((jp_hi + kN / 2 + H - 1) / H);
+                    d.tf_hi = std::min(h_hi, d.T);
+                }
+                d.regen = stat ? 0 : iir_regen_ok(b_iir, d.T, 0);
+                if (pad + step > sig_len) zero_units.push_back(u);               // stationary.py:126 leaves the tail zero
+                {   // hops per synthesis work item: run_core's choice for a [channels][n] recording in one workspace batch
+                    const long long hops = std::max(0, h_hi - h_lo), want = (long long)resident * kWarps * 4;
+                    long long run = std::max(16LL, std::min(128LL, (nch * rw.channels * hops + want - 1) / want));
+                    run += run & 1;
+                    d.run = (int)run;
+                    n_runs2 = std::max(n_runs2, (hops + run - 1) / run);
+                }
+                T_max = std::max(T_max, d.T);
+                tf_hi_max = std::max(tf_hi_max, d.tf_hi);
+                frames += d.T;
+            }
+        }
+    }
+    h->stats = b200gate_stats{};
+    h->masks_valid = false;
+    long long launches = 0;
+    CK(h, cudaMemcpyAsync(h->d_units, h->hp_units, tbytes, cudaMemcpyHostToDevice, st));
+    CK(h, cudaEventRecord(h->ev_units, st));
+    const UnitDesc* d_units = (const UnitDesc*)h->d_units;
+    if (!is_device) CK(h, cudaMemcpyAsync(h->d_in, in_lo, in_span, cudaMemcpyHostToDevice, st));
+    for (long long u : zero_units) {
+        const UnitDesc& d = h->hp_units[u];
+        CK(h, cudaMemsetAsync((char*)d.y + (size_t)d.o_lo * es, 0, (size_t)(d.o_hi - d.o_lo) * es, st));
+    }
+
+    // ---- workspace: run_core's per-unit buffers at the pitch of the longest unit ---------------------------------------
+    Geom g{};
+    g.H = H; g.C = 1; g.T = T_max; g.pad = pad;
+    const int zpairs = (T_max + 1) / 2;
+    const size_t zunit = (size_t)zpairs * 1024 * sizeof(float2);
+    const size_t per_unit = (stat ? (size_t)T_max * kFW * 4 + (size_t)kFPad * 4 + (size_t)kFW * 4 + 64
+                                  : 2 * (size_t)T_max * kFPad * 4 + 64) + 2048 + zunit;
+    double limit = p.workspace_limit_bytes;
+    if (!(limit > 0)) {
+        limit = 24.0 * 1024 * 1024 * 1024;
+        size_t free_b = 0, total_b = 0;
+        if (cudaMemGetInfo(&free_b, &total_b) == cudaSuccess)
+            limit = std::min(limit, 0.7 * ((double)free_b + (double)h->ws_bytes));
+    }
+    long long ub = std::min(U, (long long)std::max(1.0, floor(limit / (double)per_unit)));
+    for (;;) {                                                  // as run_core: halve the batch if the device cannot give it
+        if (ensure(h, (void**)&h->d_ws_buf, &h->ws_bytes, (size_t)ub * per_unit + ((size_t)8 << 20)) == B200GATE_OK) break;
+        cudaGetLastError();
+        if (ub / 2 < 1) return B200GATE_ERR_NOMEM;
+        ub /= 2;
+    }
+    if (ub < U) {                                               // equal batches
+        const long long nb = (U + ub - 1) / ub;
+        ub = std::min(ub, std::max((U + nb - 1) / nb, 1LL));
+    }
+    auto al = [](size_t v) { return (v + 255) / 256 * 256; };
+    const size_t off_rowmax = al((size_t)ub * T_max * kFW * 4);
+    const size_t off_rowflag = off_rowmax + al((size_t)ub * kFPad * 4);
+    const size_t end_stat = off_rowflag + al((size_t)ub * kFW * 4);
+    const size_t off_m0 = al((size_t)ub * T_max * kFPad * 4);
+    const size_t end_nonstat = off_m0 + al((size_t)ub * T_max * kFPad * 4);
+    const size_t off_z = al(stat ? end_stat : end_nonstat);
+    {
+        const int rc = ensure(h, (void**)&h->d_ws_buf, &h->ws_bytes, off_z + al((size_t)ub * zunit));
+        if (rc) return rc;
+    }
+    unsigned* d_bits = (unsigned*)h->d_ws_buf;
+    unsigned* d_rowmax = (unsigned*)(h->d_ws_buf + off_rowmax);
+    unsigned* d_rowflag = (unsigned*)(h->d_ws_buf + off_rowflag);
+    float* d_mag = (float*)h->d_ws_buf;
+    float* d_m0 = (float*)(h->d_ws_buf + off_m0);
+    float2* d_zcache = (float2*)(h->d_ws_buf + off_z);
+
+    CK(h, cudaMemsetAsync(h->d_cnt, 0, sizeof(Counters), st));
+    h->dbg_T = 0;
+    const Tables tb = device_tables(h);
+    const double D = (double)(nf + 1) * (nf + 1) * (nt + 1) * (nt + 1);
+    const size_t n_batches = (size_t)((U + ub - 1) / ub);
+    while (h->stage_ev.size() < 4 * n_batches) {
+        cudaEvent_t e;
+        CK(h, cudaEventCreate(&e));
+        h->stage_ev.push_back(e);
+    }
+    DebugTap dbg{};
+    dbg.ul = -1;
+    const long long hops = n_runs2;                             // (> 0: some unit has output hops)
+    size_t bi = 0;
+    cudaEventRecord(h->ev0, st);
+    for (long long u0 = 0; u0 < U; u0 += ub, ++bi) {
+        const int nu = (int)std::min(ub, U - u0);
+        g.u0 = (int)u0;
+        g.n_units = nu;
+        // frames per analysis work item, sized as in run_core (the synthesis work items: UnitDesc::run)
+        long long want = (long long)(stat ? h->num_sm * B200_K1_MINBLOCKS : resident) * kWarps * 4;
+        long long run1 = std::max(8LL, std::min(64LL, ((long long)nu * T_max + want - 1) / want));
+        run1 += run1 & 1;
+        const int n_runs1 = (int)((T_max + run1 - 1) / run1);
+        K2Args a2{};
+        a2.g = g; a2.tb = tb; a2.zcache = d_zcache; a2.zpairs = zpairs; a2.nt = nt; a2.dbg = dbg; a2.units = d_units;
+        a2.n_runs = (int)n_runs2;
+        const unsigned grid2 = (unsigned)grid_1d((long long)nu * a2.n_runs, kWarps, resident);
+        cudaEventRecord(h->stage_ev[4 * bi + 0], st);
+        if (stat) {
+            CK(h, cudaMemsetAsync(d_rowmax, 0, (size_t)nu * kFPad * 4, st));
+            CK(h, cudaMemsetAsync(h->d_need_rowmax, 0, sizeof(unsigned), st));
+            K1Args a1{};
+            a1.g = g; a1.tb = tb; a1.bits = d_bits; a1.rowmax = d_rowmax; a1.cnt = h->d_cnt; a1.dbg = dbg;
+            a1.zcache = d_zcache; a1.zpairs = zpairs; a1.z_lo = tf_lo; a1.z_hi = tf_hi_max + 1; a1.units = d_units;
+            a1.run = (int)run1; a1.n_runs = n_runs1;
+            a1.need_rowmax = h->d_need_rowmax;
+            a1.min_floor4 = (float)(4.0 * h->min_floor_amp * h->min_floor_amp);
+            const unsigned grid1 = (unsigned)grid_1d((long long)nu * n_runs1, kWarps, h->num_sm * B200_K1_MINBLOCKS);
+            B200_WITH_DTYPE(dtype, { auto kern_ = k1_analyze<8, T, false, true>;
+                B200_LAUNCH(kern_, dim3(grid1), dim3(kThreads), k1_smem_floats() * 4, st, a1); });
+            a1.guard = h->d_need_rowmax;                        // the row-maximum fallback, as in run_core
+            a1.zcache = nullptr;
+            B200_WITH_DTYPE(dtype, { auto kern_ = k1_analyze<8, T, true, true>;
+                B200_LAUNCH(kern_, dim3(grid1), dim3(kThreads), k1_smem_floats() * 4, st, a1); });
+            B200_LAUNCH(k_rowfloor, dim3(grid_1d((long long)nu * kFW, 256, 1 << 30)), dim3(256), 0, st, nu,
+                        (const unsigned*)d_rowmax, (const float*)h->d_floor4, d_rowflag, h->d_cnt);
+            launches += 3;
+            cudaEventRecord(h->stage_ev[4 * bi + 1], st);
+            cudaEventRecord(h->stage_ev[4 * bi + 2], st);
+            if (hops > 0) {
+                a2.pD = (float)(p.prop_decrease / D);
+                a2.one_minus_p = (float)(1.0 - p.prop_decrease);
+                a2.bits = d_bits; a2.rowflag = d_rowflag;
+                set_k2c_smoothing_taps(a2, nf);
+                if (a2.one_minus_p != 0.f) {
+                    B200_WITH_DTYPE(dtype, { auto kern2 = k2c_synthesize<8, kMaskBitsBlend, T, true>;
+                        B200_LAUNCH(kern2, dim3(grid2), dim3(kThreads), k2c_smem_bytes<kMaskBitsBlend>(), st, a2); });
+                } else {
+                    B200_WITH_DTYPE(dtype, { auto kern2 = k2c_synthesize<8, kMaskBits, T, true>;
+                        B200_LAUNCH(kern2, dim3(grid2), dim3(kThreads), k2c_smem_bytes<kMaskBits>(), st, a2); });
+                }
+                ++launches;
+            }
+        } else {
+            K1nArgs a1{};
+            a1.g = g; a1.tb = tb; a1.mag = d_mag; a1.dbg = dbg; a1.zcache = d_zcache; a1.zpairs = zpairs;
+            a1.z_lo = tf_lo; a1.z_hi = tf_hi_max + 1; a1.units = d_units;
+            a1.run = (int)run1; a1.n_runs = n_runs1;
+            B200_WITH_DTYPE(dtype, { auto kern_ = k1n_magnitude<8, T, true>;
+                B200_LAUNCH(kern_, dim3(grid_1d((long long)nu * n_runs1, kWarps, resident)), dim3(kThreads),
+                            k1n_smem_floats() * 4, st, a1); });
+            cudaEventRecord(h->stage_ev[4 * bi + 1], st);
+            IirArgs ia{};
+            ia.n_units = nu; ia.T = T_max; ia.F = kF; ia.FPad = kFPad; ia.b = b_iir;
+            ia.n_mult = (float)p.thresh_n_mult; ia.slope = (float)p.sigmoid_slope;
+            ia.mag = d_mag; ia.m0 = d_m0; ia.units = d_units + u0;    // (regen: each unit's own, UnitDesc::regen)
+            { auto kern_ = k_iir_sigmoid<kFPad, true>;
+              B200_LAUNCH(kern_, dim3(grid_1d((long long)nu * kFPad, 128, 1 << 30)), dim3(128), 0, st, ia); }
+            launches += 2;
+            if (tf_hi_max > tf_lo) {
+                SmoothFArgs sa{};
+                sa.n_units = nu; sa.T = T_max; sa.nf = nf; sa.nt = nt; sa.tf_lo = tf_lo; sa.tf_hi = tf_hi_max; sa.TT = 32;
+                sa.F = kF; sa.FPad = kFPad;
+                sa.p = (float)p.prop_decrease; sa.one_minus_p = (float)(1.0 - p.prop_decrease);
+                sa.m0 = d_m0; sa.m2 = d_mag; sa.units = d_units + u0;
+                launch_smooth_float<true>(sa, nf, nt, tf_lo, tf_hi_max, nu, 0, st);      // (extents checked on entry)
+                ++launches;
+            }
+            cudaEventRecord(h->stage_ev[4 * bi + 2], st);
+            if (hops > 0 && tf_hi_max > tf_lo) {
+                a2.fmask = d_mag;
+                B200_WITH_DTYPE(dtype, { auto kern2 = k2c_synthesize<8, kMaskF32, T, true>;
+                    B200_LAUNCH(kern2, dim3(grid2), dim3(kThreads), k2c_smem_bytes<kMaskF32>(), st, a2); });
+                ++launches;
+            }
+        }
+        cudaEventRecord(h->stage_ev[4 * bi + 3], st);
+        CK(h, cudaGetLastError());
+    }
+    cudaEventRecord(h->ev1, st);
+    if (!is_device) CK(h, cudaMemcpyAsync((void*)out_lo, h->d_out, out_span, cudaMemcpyDeviceToHost, st));
+    CK(h, cudaMemcpyAsync(h->h_cnt, h->d_cnt, sizeof(Counters), cudaMemcpyDeviceToHost, st));
+    CK(h, cudaEventRecord(h->ev_done, st));
+    h->stats.units = U;
+    h->stats.frames = frames;
+    h->stats.kernel_launches = launches;
+    h->stats_pending = true;
+    h->pend_batches = n_batches;
+    if (!is_device) {                            // host rows: the results must be in place on return
+        const int rc = resolve_stats(h);
+        if (rc) return rc;
+    }
+    return B200GATE_OK;
 }
 
 int b200gate_mask_store_bytes(b200gate_handle* h, int64_t C, int64_t N, int64_t* bytes) {

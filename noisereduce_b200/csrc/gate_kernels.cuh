@@ -50,6 +50,22 @@ struct Geom {
     int u0, n_units;        // this batch: units [u0, u0 + n_units); u = chunk * C + channel
 };
 
+// b200gate_run_rows: every unit of a call carries its own geometry and row pointers (kernels templated with ROWS read
+// them from units[g.u0 + ul]; Geom then holds what the units share -- H, pad, u0, n_units -- and T = the longest unit's
+// frame count, the pitch of every per-unit buffer).
+struct UnitDesc {
+    const void* x;          // sample 0 of the unit's input row
+    void* y;                // sample 0 of its output row
+    long long n_total;      // samples of the row
+    long long i1;           // first sample of the padded span (may be < 0)
+    long long Lp;           // padded span length
+    long long o_lo, o_hi;   // samples of the row this unit writes
+    int T;                  // frames: Lp / H + 1
+    int tf_hi;              // masks are needed for frames [tf_lo, tf_hi) (tf_lo is the same for every unit)
+    int regen;              // k_iir_sigmoid: iir_regen_ok of this unit's T
+    int run;                // k2c_synthesize: output hops per work item, as run_core sizes them for this unit's recording
+};
+
 struct Tables {              // device pointers, built once per handle
     const float* wa;         // [N] analysis window / sum(w)
     const float* ws;         // [N] synthesis window * sum(w) / N
@@ -336,6 +352,7 @@ struct K1Args {
                                // row-maximum fallback behind k1_analyze<.., false> or k1d_analyze, gate_dual.cuh)
     unsigned* need_rowmax;     // k1_analyze<.., false>: device flag raised when a frame could reach its top_db floor
     float min_floor4;          // min over bins of 4 * (10^((thresh + top_db)/20) - eps)^2
+    const UnitDesc* units;     // ROWS instantiations: the call's unit table
 };
 
 // One pair's sample window (32 + 8 rows of 32 samples) as the 16-byte-aligned span that covers it: up to 16 bytes more.
@@ -349,7 +366,7 @@ constexpr int k1_smem_floats() {
 // raises need_rowmax when a pair's energy could reach the lowest floor (|X_k|^2 <= N ||frame||^2), and the host then runs
 // the ROWMAX = true instantiation behind it (guarded by that flag) for the maxima.  That instantiation loads the samples
 // directly and tracks the maxima of every bin; run alone it is the whole analysis.
-template <int HR, typename T, bool ROWMAX = false>
+template <int HR, typename T, bool ROWMAX = false, bool ROWS = false>
 __global__ void __launch_bounds__(kThreads, B200_K1_MINBLOCKS) k1_analyze(const K1Args a) {
     static_assert(32 * (32 + HR) * 4 + 16 <= kK1WinBytes, "sample window must fit the buffer");
     constexpr bool kBulk = !ROWMAX && sizeof(T) <= 4;   // float32 / int16 windows (float64: direct loads)
@@ -395,27 +412,34 @@ __global__ void __launch_bounds__(kThreads, B200_K1_MINBLOCKS) k1_analyze(const 
         run_ += step_run;
         if (run_ >= a.n_runs) { run_ -= a.n_runs; ++ul_; }
     };
-    // sample row and chunk origin (global index of chunk sample 0) of a local unit
+    // sample row and chunk origin (global index of chunk sample 0) of a local unit; ROWS: also its span, row length and frames
     auto unit_row = [&](int ul_, const T*& xrow, long long& i1) {
         const int u = g.u0 + ul_;
+        if (ROWS) {
+            xrow = static_cast<const T*>(a.units[u].x);
+            i1 = a.units[u].i1;
+            return;
+        }
         const int ic = u / g.C, c = u - ic * g.C;
         i1 = (long long)ic * g.step - g.pad;
         xrow = static_cast<const T*>(a.x) + (long long)c * g.in_stride;
     };
+    auto unit_Lp = [&](int ul_) -> long long { return ROWS ? a.units[g.u0 + ul_].Lp : g.Lp; };
+    auto unit_n = [&](int ul_) -> long long { return ROWS ? a.units[g.u0 + ul_].n_total : g.n_total; };
     // Request the window of pair (tt, tt + 1) of a unit into this warp's buffer when it lies inside the chunk and the
     // recording and the 16-byte-aligned span covering it lies inside the samples the chunk reads,
     // [max(0, i1), min(n_total, i1 + Lp)).  (Bounding it by the row instead let the aligned span reach past the rows a
     // caller staged or streamed -- [w_lo, w_hi) of b200gate_run -- by up to 15 bytes at either end.)  Returns the
     // window's element offset in the buffer, or -1: the pair is then loaded directly.  Warp-uniform; every lane has
     // finished reading the buffer.
-    auto request = [&](const T* xr_, long long i1_, int tt) -> int {
+    auto request = [&](const T* xr_, long long i1_, long long Lp_, long long n_, int tt) -> int {
         if (!kBulk) return -1;
         const long long bb = (long long)tt * H - kN / 2;
-        if (!pair_window_interior<HR>(bb, i1_, g.Lp, g.n_total)) return -1;
+        if (!pair_window_interior<HR>(bb, i1_, Lp_, n_)) return -1;
         const unsigned long long src = reinterpret_cast<unsigned long long>(xr_ + i1_ + bb);
         const unsigned long long lo = src & ~15ull;
         const unsigned long long hi = (src + 32 * (32 + HR) * sizeof(T) + 15) & ~15ull;
-        const long long r_lo = i1_ > 0 ? i1_ : 0, r_hi = i1_ + g.Lp < g.n_total ? i1_ + g.Lp : g.n_total;
+        const long long r_lo = i1_ > 0 ? i1_ : 0, r_hi = i1_ + Lp_ < n_ ? i1_ + Lp_ : n_;
         if (lo < reinterpret_cast<unsigned long long>(xr_ + r_lo) || hi > reinterpret_cast<unsigned long long>(xr_ + r_hi))
             return -1;
         fence_proxy_async_smem();
@@ -433,15 +457,16 @@ __global__ void __launch_bounds__(kThreads, B200_K1_MINBLOCKS) k1_analyze(const 
         const T* xr_;
         long long i1_;
         unit_row(ul, xr_, i1_);
-        woff = request(xr_, i1_, run * a.run);
+        woff = request(xr_, i1_, unit_Lp(ul), unit_n(ul), run * a.run);
     }
 
     for (; item < n_items; item += item_stride, next_item(ul, run)) {
         const T* xrow;
         long long i1;
         unit_row(ul, xrow, i1);
+        const long long Lp_u = unit_Lp(ul), n_u = unit_n(ul);
         const int t0 = run * a.run;
-        const int t1 = min(t0 + a.run, g.T);
+        const int t1 = min(t0 + a.run, ROWS ? a.units[g.u0 + ul].T : g.T);
         float mx[ROWMAX ? kFW : 1];
         if (ROWMAX) {
 #pragma unroll
@@ -460,18 +485,18 @@ __global__ void __launch_bounds__(kThreads, B200_K1_MINBLOCKS) k1_analyze(const 
 #pragma unroll
                 for (int r = 0; r < 32 + HR; ++r) xr[r] = (float)wp[32 * r];
             } else {
-                load_pair_rows<HR>(xr, xrow, base, i1, g.Lp, g.n_total, lane);
+                load_pair_rows<HR>(xr, xrow, base, i1, Lp_u, n_u, lane);
             }
             if (kBulk) {                                     // the next window streams in behind this pair's transform
                 if (t + 2 < t1) {
-                    woff = request(xrow, i1, t + 2);
+                    woff = request(xrow, i1, Lp_u, n_u, t + 2);
                 } else if (item + item_stride < n_items) {   // the first window of the warp's next work item
                     int uln = ul, runn = run;
                     next_item(uln, runn);
                     const T* xr_;
                     long long i1_;
                     unit_row(uln, xr_, i1_);
-                    woff = request(xr_, i1_, runn * a.run);
+                    woff = request(xr_, i1_, unit_Lp(uln), unit_n(uln), runn * a.run);
                 } else {
                     woff = -1;
                 }
@@ -548,7 +573,7 @@ __global__ void __launch_bounds__(kThreads, B200_K1_MINBLOCKS) k1_analyze(const 
                         while (m) {
                             const int src = __ffs((int)m) - 1;
                             m &= m - 1;
-                            const int r = recheck_bin_fp64(xrow, base + (long long)fr * H, i1, g.Lp, g.n_total,
+                            const int r = recheck_bin_fp64(xrow, base + (long long)fr * H, i1, Lp_u, n_u,
                                                            src + 32 * q, a.tb.wa64, a.tb.cs64, a.tb.thr2_64, lane);
                             ++nre;
                             if (r == 0) { ++nun; continue; }
@@ -854,6 +879,7 @@ struct K2Args {
     // padded span goes to adj[ul][0, Lp) (chunk-local index), which k_adj_gather sums across units.
     float* adj;
     long long adj_pitch;
+    const UnitDesc* units;         // k2c_synthesize<.., ROWS = true>: the call's unit table
 };
 
 constexpr int k2_smem_floats(int H) { return 2 * kN + 2 * kN + H + kFPad + kWarps * kExchFloats + 8 + kWarps * 2 * kN; }
@@ -1183,11 +1209,12 @@ struct K1nArgs {
     float2* zcache;            // optional, as in K1Args
     int zpairs;
     int z_lo, z_hi;
+    const UnitDesc* units;     // ROWS instantiations: the call's unit table
 };
 
 constexpr int k1n_smem_floats() { return kN + 2 * kN + kWarps * kExchFloats; }
 
-template <int HR, typename T>
+template <int HR, typename T, bool ROWS = false>
 __global__ void __launch_bounds__(kThreads, 3) k1n_magnitude(const K1nArgs a) {
     B200_DYN_SMEM(float, smem);
     float* s_wa = smem;
@@ -1210,15 +1237,18 @@ __global__ void __launch_bounds__(kThreads, 3) k1n_magnitude(const K1nArgs a) {
         const int run = (int)(item - (long long)ul * a.n_runs);
         const int u = g.u0 + ul;
         const int ic = u / g.C, c = u - ic * g.C;
-        const long long i1 = (long long)ic * g.step - g.pad;
-        const T* xrow = static_cast<const T*>(a.x) + (long long)c * g.in_stride;
+        const UnitDesc* d = ROWS ? a.units + u : nullptr;        // ROWS: the unit's own row, span and frames
+        const long long i1 = ROWS ? d->i1 : (long long)ic * g.step - g.pad;
+        const T* xrow = ROWS ? static_cast<const T*>(d->x) : static_cast<const T*>(a.x) + (long long)c * g.in_stride;
+        const long long Lp_u = ROWS ? d->Lp : g.Lp, n_u = ROWS ? d->n_total : g.n_total;
+        const int T_u = ROWS ? d->T : g.T;
         const int t0 = run * a.run;
-        const int t1 = min(t0 + a.run, g.T);
+        const int t1 = min(t0 + a.run, T_u);
         for (int t = t0; t < t1; t += 2) {
             const bool vb = (t + 1 < t1);
             const long long base = (long long)t * H - kN / 2;
             float re[32], im[32];
-            load_frame_pair<HR>(re, im, xrow, base, i1, g.Lp, g.n_total, s_wa, lane, vb);
+            load_frame_pair<HR>(re, im, xrow, base, i1, Lp_u, n_u, s_wa, lane, vb);
             warp_fft1024(re, im, tile, s_tw, lane);
             if (a.zcache && t >= a.z_lo && t < a.z_hi) {
                 float2* zp = a.zcache + ((long long)ul * a.zpairs + (t >> 1)) * 1024 + lane;
@@ -1262,9 +1292,10 @@ struct IirArgs {
     int regen;                 // 1: regenerate the forward sweep in the backward pass instead of storing it
     const float* mag;          // [n_units][T][FPad]
     float* m0;                 // [n_units][T][FPad]: forward sweep, then overwritten by the sigmoid mask
+    const UnitDesc* units;     // ROWS instantiations: units + (first unit of the batch); T is then the pitch only
 };
 
-template <int FP>                                       // padded row pitch: 544 (n_fft 1024) or 1056 (n_fft 2048)
+template <int FP, bool ROWS = false>                    // padded row pitch: 544 (n_fft 1024) or 1056 (n_fft 2048)
 __global__ void __launch_bounds__(128) k_iir_sigmoid(const IirArgs a) {
     const int FF = a.F;
     const long long idx = (long long)blockIdx.x * blockDim.x + threadIdx.x;
@@ -1272,8 +1303,11 @@ __global__ void __launch_bounds__(128) k_iir_sigmoid(const IirArgs a) {
     const int ul = (int)(idx / FP), f = (int)(idx - (long long)ul * FP);
     const float* __restrict__ A = a.mag + (long long)ul * a.T * FP + f;
     float* M = a.m0 + (long long)ul * a.T * FP + f;
+    // ROWS: the unit's own frame count, and its own choice between the two (differently rounding) variants below
+    const int T = ROWS ? a.units[ul].T : a.T;
+    const int regen = ROWS ? a.units[ul].regen : a.regen;
     if (f >= FF) {
-        for (int t = 0; t < a.T; ++t) M[(long long)t * FP] = 0.f;
+        for (int t = 0; t < T; ++t) M[(long long)t * FP] = 0.f;
         return;
     }
     // The recurrence state stays in float64 (the filter pole 1 - b ~ 0.995 accumulates rounding over hundreds of
@@ -1287,7 +1321,6 @@ __global__ void __launch_bounds__(128) k_iir_sigmoid(const IirArgs a) {
     constexpr int kB = 8;
     const double b = a.b, omb = 1.0 - a.b;
     const float n_mult = a.n_mult, slope = a.slope;
-    const int T = a.T;
     auto sigmoid_mask = [&](double x, double sm) -> float {
         const float num = (float)(x - sm);                     // |X| - S without float32 cancellation
         const float r = num * __frcp_rn((float)sm);
@@ -1311,7 +1344,7 @@ __global__ void __launch_bounds__(128) k_iir_sigmoid(const IirArgs a) {
         }
     };
     double s = (double)A[0];
-    if (a.regen) {
+    if (regen) {
         // The forward sweep is not stored: the backward sweep regenerates it by the inverse recurrence
         // fwd[t-1] = (fwd[t] - b x[t]) / (1 - b) in float64.  One read of |X| less, no forward write.  Its error
         // grows by 1/(1 - b) per step, and what matters is the error RELATIVE TO S, which in a quiet stretch can be
@@ -1410,6 +1443,8 @@ struct SmoothFArgs {
     float p, one_minus_p;
     const float* m0;           // [n_units][T][FPad]
     float* m2;                 // [n_units][T][FPad]
+    const UnitDesc* units;     // ROWS instantiations: units + (first unit of the batch); T is then the pitch only and
+                               // tf_hi the largest of the batch
 };
 __host__ __device__ inline int smoothf_cpitch(int FPad, int nf) { return FPad + 2 * nf + 1; }
 inline size_t smoothf_smem_bytes(int TT, int FPad, int nf) { return (size_t)TT * smoothf_cpitch(FPad, nf) * 4; }
@@ -1460,6 +1495,7 @@ __global__ void __launch_bounds__(256) k_smooth_f(const SmoothFArgs a) {
 // once per strip and written once.
 inline size_t smooths_smem_bytes(int FPad, int nf, int nt) { return ((size_t)(2 * nt + 1) * FPad + FPad + 2 * nf + 8) * 4; }
 
+template <bool ROWS = false>
 __global__ void __launch_bounds__(288) k_smooth_stream(const SmoothFArgs a) {
     B200_DYN_SMEM(float, s_buf);
     const int FP = a.FPad, FF = a.F, nt = a.nt, nf = a.nf, R = 2 * nt + 1;
@@ -1467,14 +1503,15 @@ __global__ void __launch_bounds__(288) k_smooth_stream(const SmoothFArgs a) {
     float* ring = s_buf;                     // [R][FP]
     float* row = s_buf + (size_t)R * FP;     // [nf | FP | nf]
     const int ul = blockIdx.y;
+    const int T = ROWS ? a.units[ul].T : a.T, tf_hi = ROWS ? a.units[ul].tf_hi : a.tf_hi;
     const int t_begin = a.tf_lo + blockIdx.x * a.TT;
-    if (t_begin >= a.tf_hi) return;
-    const int t_end = min(t_begin + a.TT, a.tf_hi);
+    if (t_begin >= tf_hi) return;
+    const int t_end = min(t_begin + a.TT, tf_hi);
     const float* src = a.m0 + (long long)ul * a.T * FP;
     float* dst = a.m2 + (long long)ul * a.T * FP;
     for (int i = tid; i < FP + 2 * nf; i += G) row[i] = 0.f;
     auto load_row = [&](int t, int slot) {
-        const bool in = t >= 0 && t < a.T;
+        const bool in = t >= 0 && t < T;
 #pragma unroll
         for (int j = 0; j < 4; ++j) {
             const int bin = tid + j * G;
@@ -1526,7 +1563,7 @@ __global__ void __launch_bounds__(288) k_smooth_stream(const SmoothFArgs a) {
 // out[f] = sum_{g=f-nf..f} b1[g] reaches nf bins to the left); bins >= F hold zeros, and FPad - F >= 12.
 inline size_t smoothb_smem_bytes(int FPad, int nt) { return ((size_t)(2 * nt + 1) * FPad + (FPad + 32) + (FPad + 16)) * 4; }
 
-template <int NF>
+template <int NF, bool ROWS = false>
 __global__ void __launch_bounds__(288) k_smooth_box(const SmoothFArgs a) {
     static_assert(NF >= 1 && NF <= 12, "box smoothing handles 1 <= nf <= 12");
     B200_DYN_SMEM(float, s_buf);
@@ -1536,16 +1573,17 @@ __global__ void __launch_bounds__(288) k_smooth_box(const SmoothFArgs a) {
     float* rowA = s_buf + (size_t)R * FP;                  // [16 | FP | 16]
     float* rowB = rowA + FP + 32;                          // [FP + 16]
     const int ul = blockIdx.y;
+    const int T = ROWS ? a.units[ul].T : a.T, tf_hi = ROWS ? a.units[ul].tf_hi : a.tf_hi;
     const int t_begin = a.tf_lo + blockIdx.x * a.TT;
-    if (t_begin >= a.tf_hi) return;
-    const int t_end = min(t_begin + a.TT, a.tf_hi);
+    if (t_begin >= tf_hi) return;
+    const int t_end = min(t_begin + a.TT, tf_hi);
     const float* src = a.m0 + (long long)ul * a.T * FP;
     float* dst = a.m2 + (long long)ul * a.T * FP;
     for (int i = tid; i < 2 * FP + 48; i += G) rowA[i] = 0.f;          // rowA and rowB are contiguous
     const int b0 = 4 * tid;
     auto fetch_row = [&](int t) -> float4 {
         float4 v = make_float4(0.f, 0.f, 0.f, 0.f);
-        if (t >= 0 && t < a.T) {
+        if (t >= 0 && t < T) {
             v = __ldg(reinterpret_cast<const float4*>(src + (long long)t * FP + b0));
             if (b0 + 0 >= FF) v.x = 0.f;
             if (b0 + 1 >= FF) v.y = 0.f;

@@ -104,7 +104,7 @@ __device__ __forceinline__ void k2c_freq_taps(const unsigned char* rows, unsigne
 #ifndef B200_K2C_MINBLOCKS
 #define B200_K2C_MINBLOCKS 3
 #endif
-template <int HR, int MK, typename T>
+template <int HR, int MK, typename T, bool ROWS = false>
 __global__ void __launch_bounds__(kThreads, B200_K2C_MINBLOCKS) k2c_synthesize(const K2Args a) {
     constexpr int NH = 32 / HR;             // frames overlapping one hop (win / hop)
     constexpr int MB = k2c_mask_bytes<MK>();
@@ -154,21 +154,27 @@ __global__ void __launch_bounds__(kThreads, B200_K2C_MINBLOCKS) k2c_synthesize(c
         const int run = (int)(item - (long long)ul * a.n_runs);
         const int u = g.u0 + ul;
         const int ic = u / g.C, c = u - ic * g.C;
-        const long long i1 = (long long)ic * g.step - g.pad;
-        long long out_len = g.n_total - (long long)ic * g.step;
-        if (out_len > g.step) out_len = g.step;
+        const UnitDesc* ud = ROWS ? a.units + u : nullptr;           // ROWS: the unit's own span and frames
+        const long long i1 = ROWS ? ud->i1 : (long long)ic * g.step - g.pad;
+        long long out_len = ROWS ? ud->o_hi - ud->o_lo : g.n_total - (long long)ic * g.step;
+        if (!ROWS && out_len > g.step) out_len = g.step;
+        const int T_u = ROWS ? ud->T : g.T;                          // (g.T stays the pitch of the per-unit buffers)
         long long jp_hi = g.pad + out_len;
-        const long long sig_len = (long long)(g.T - 1) * H;          // istft output length
+        const long long sig_len = (long long)(T_u - 1) * H;          // istft output length
         if (jp_hi > sig_len) jp_hi = sig_len;                        // beyond it the reference leaves zeros
         if (jp_hi <= g.pad) continue;
         const long long jlo = g.pad + kN / 2, jhi = jp_hi + kN / 2;
         const int h_lo = (int)(jlo / H), h_hi = (int)((jhi + H - 1) / H);
-        const int hs = h_lo + run * a.run;
-        const int he = min(hs + a.run, h_hi);
+        // ROWS: the recording's own work-item length.  A work item that ends on an odd frame transforms its last frame
+        // alone instead of packed with its successor, which rounds differently in the last bit, so the hops at work-item
+        // seams depend on this length; each unit uses the one b200gate_run would use for its recording.
+        const int run_len = ROWS ? ud->run : a.run;
+        const int hs = h_lo + run * run_len;
+        const int he = min(hs + run_len, h_hi);
         if (hs >= he) continue;
         const int t_start = max(0, hs - (NH - 1)) & ~1;              // k1 packed frames (2j, 2j+1): walk the same pairs
-        const int t_last = min(he - 1, g.T - 1);
-        T* yrow = static_cast<T*>(a.y) + (long long)c * g.out_stride;
+        const int t_last = min(he - 1, T_u - 1);
+        T* yrow = ROWS ? static_cast<T*>(a.units[u].y) : static_cast<T*>(a.y) + (long long)c * g.out_stride;
         const float2* zunit = a.zcache + (long long)ul * a.zpairs * 1024;
         const unsigned short* munit = (MK == kMaskF32 || kBits) ? nullptr : a.num + (long long)ul * a.zpairs * (2 * kFPad);
         const float* funit = (MK == kMaskF32) ? a.fmask + (long long)ul * g.T * kFPad : nullptr;
@@ -203,7 +209,7 @@ __global__ void __launch_bounds__(kThreads, B200_K2C_MINBLOCKS) k2c_synthesize(c
         // this lane's decisions of frame tau: x = its 16 bins (4 bits per group), y = bins 512..515 (lane 0 only);
         // frames before tau_s count as zero, as in k_smooth_packed
         auto fetch = [&](int tau, uint2 fl) -> uint2 {
-            if (tau < tau_s || tau < 0 || tau >= g.T) return uint2{0u, 0u};
+            if (tau < tau_s || tau < 0 || tau >= T_u) return uint2{0u, 0u};
             const unsigned* row = bunit + (long long)tau * kFW;
             const unsigned w = __ldg(row + (lane >> 1)) | fl.x;
             const unsigned w5 = (__ldg(row + 16) | fl.y) & 0xFu;
@@ -293,8 +299,8 @@ __global__ void __launch_bounds__(kThreads, B200_K2C_MINBLOCKS) k2c_synthesize(c
                     pb = vb ? pa : 0.f;
                     cb = vb ? ca : 0.f;
                     if (kBlend) {
-                        eta = 0.5f * a.one_minus_p * time_edge(t, g.T, a.nt);
-                        etb = vb ? 0.5f * a.one_minus_p * time_edge(t + 1, g.T, a.nt) : 0.f;
+                        eta = 0.5f * a.one_minus_p * time_edge(t, T_u, a.nt);
+                        etb = vb ? 0.5f * a.one_minus_p * time_edge(t + 1, T_u, a.nt) : 0.f;
                     }
                 }
                 auto half_masks = [&](int kk, float& ma, float& mb) {      // m_a / 2, m_b / 2 at bin kk
@@ -406,7 +412,7 @@ __global__ void __launch_bounds__(kThreads, B200_K2C_MINBLOCKS) k2c_synthesize(c
             // hops t and t+1 are now complete (all frames <= t+1 have been added)
             {
                 const long long jp0 = (long long)t * H - kN / 2;             // chunk-local index of row 0, lane 0
-                if (t >= hs && t + 1 < he && t >= NH - 1 && t + 1 <= g.T - 1 && jp0 >= g.pad &&
+                if (t >= hs && t + 1 < he && t >= NH - 1 && t + 1 <= T_u - 1 && jp0 >= g.pad &&
                     jp0 + 2 * H <= jp_hi) {
                     // both hops interior and fully inside the chunk centre: 2*HR coalesced row stores
                     T* dst = yrow + i1 + jp0 + lane;
@@ -425,13 +431,13 @@ __global__ void __launch_bounds__(kThreads, B200_K2C_MINBLOCKS) k2c_synthesize(c
                         const long long jp = (long long)hop * H + ro - kN / 2;   // chunk-local output index
                         if (jp < g.pad || jp >= jp_hi) continue;
                         float inv;
-                        if (hop >= NH - 1 && hop <= g.T - 1) {
+                        if (hop >= NH - 1 && hop <= T_u - 1) {
                             inv = a.tb.invn[ro];
                         } else {                                                  // first / last hops
                             float nrm = 0.f;
                             for (int i = 0; i < NH; ++i) {
                                 const int tf = hop - i;
-                                if (tf >= 0 && tf <= g.T - 1) {
+                                if (tf >= 0 && tf <= T_u - 1) {
                                     const float w = s_ws[i * H + ro] * a.tb.ws_to_w;
                                     nrm = fmaf(w, w, nrm);
                                 }
