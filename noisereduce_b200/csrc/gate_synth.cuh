@@ -191,7 +191,7 @@ __global__ void __launch_bounds__(kThreads, B200_K2C_MINBLOCKS) k2c_synthesize(c
                 const bool vb2 = tt + 1 <= t_last;
                 const unsigned mbytes = kBits ? 0u : ((MK == kMaskF32 && !vb2) ? (unsigned)(kFPad * 4) : (unsigned)MB);
                 mbar_expect_tx(bar, (unsigned)(kN * 8) + mbytes);
-                bulk_g2s(zbuf, zunit + (long long)(tt >> 1) * 1024, kN * 8, bar);
+                bulk_g2s_once(zbuf, zunit + (long long)(tt >> 1) * 1024, kN * 8, bar);
                 if (MK == kMaskF32) bulk_g2s(mbuf, funit + (long long)tt * kFPad, mbytes, bar);
                 else if (!kBits) bulk_g2s(mbuf, munit + (long long)(tt >> 1) * (2 * kFPad), mbytes, bar);
             }
