@@ -174,7 +174,7 @@ int b200gate_torch_apply_masks(b200gate_handle* h, const void* in, void* out, in
 int b200gate_run(b200gate_handle* h, const void* in, void* out, int dtype, int64_t C, int64_t N,
                  int64_t in_stride, int64_t out_stride, int is_device, void* cuda_stream);
 
-/* Rows of different lengths in one call (numpy surface): every row is a recording of its own, one channel of `n`
+/* Rows of different lengths in one call.  Numpy surface: every row is a recording of its own, one channel of `n`
  * samples, and out[0, n) of row r holds exactly what b200gate_run writes for that channel of its [channels][n] recording -- the chunk
  * grid, the padded span, the frame count and everything derived from them (smoothing edges, overlap-add edge norm,
  * top_db row maxima, the non-stationary follower's sweeps and its choice between regenerating and storing the forward
@@ -185,11 +185,23 @@ int b200gate_run(b200gate_handle* h, const void* in, void* out, int dtype, int64
  * waiting for the device.  Host rows must lie in one buffer each way: they travel as the span that covers them, one copy
  * in and one copy out (bytes of the output span between rows are overwritten), and the call returns with the result in
  * place.  b200gate_get_stats counts the units of all rows and their own frames.
- * B200GATE_ERR_STATE: a torch surface, an open stream, a mask store set, a range mode other than 0, a stationary gate
- * without thresholds.  B200GATE_ERR_ARG: a geometry other than n_fft = win_length = 1024, hop_length = 256; non-zero
- * path_flags; smoothing extents beyond the in-synthesis smoothing (stationary: n_grad_time > 13 or n_grad_freq > 17) or
- * beyond the streaming float-mask smoothing; n <= 0, channels <= 0, a null pointer, out overlapping in; scattered host rows.  A refused
- * call changes nothing on the handle. */
+ * Torch surface (B200GATE_SURFACE_TORCH): every row is one TorchGate row of n >= 2 win_length float32 samples, filtered
+ * as b200gate_run filters a [1][n] input -- one unit with origin 0 and no chunk padding, zeros outside [0, n), T = n / hop
+ * + 1 frames, statistics over the row's own frames (or the thresholds of b200gate_torch_set_noise: one row for every row
+ * of the call, or row r for row r) -- and out[0, (n / hop) * hop + (n_fft & 1)) of row r holds the result.  Device rows
+ * are written there and nowhere else.  Host rows travel as the output span that covers them, zeroed on the device first:
+ * every byte of that span outside the rows' results (samples [(n / hop) * hop, n) of a row, gaps between rows) is
+ * overwritten with zeros.  `channels` keeps its meaning (TorchGate passes 1).  Stationary smoothing extents beyond the
+ * in-synthesis smoothing run through a separate numerator kernel, up to the 16-bit numerator limit below.  The masks of a call that fits one workspace batch stay on the handle for
+ * b200gate_torch_apply_masks_rows.
+ * B200GATE_ERR_STATE: the TORCH_CHUNKED surface, an open stream, a mask store set, a range mode other than 0, a
+ * numpy-surface stationary gate without thresholds.  B200GATE_ERR_ARG: a geometry other than n_fft = win_length = 1024,
+ * hop_length = 256; a smoothing filter that b200gate_create sent to the general family ((n_grad_freq + 1)^2
+ * (n_grad_time + 1)^2 > 65535, or either extent > 64); non-zero path_flags; smoothing extents beyond the in-synthesis smoothing (numpy surface, stationary:
+ * n_grad_time > 13 or n_grad_freq > 17) or beyond the streaming float-mask smoothing; n <= 0, channels <= 0, a null
+ * pointer, out overlapping in; scattered host rows; on the torch surface a dtype other than B200GATE_F32, a row shorter
+ * than 2 win_length ("x must be bigger than ..."), xn thresholds of more than one row that are not one per row.  A
+ * refused call changes nothing on the handle. */
 typedef struct b200gate_row {
     const void* in; void* out; int64_t n;
     int64_t channels;   /* rows of the recording this row is a channel of (>= 1).  Sizes the synthesis work items as
@@ -198,6 +210,12 @@ typedef struct b200gate_row {
 } b200gate_row;
 int b200gate_run_rows(b200gate_handle* h, const b200gate_row* rows, int64_t n_rows, int dtype, int is_device,
                       void* cuda_stream);
+/* Torch surface: the rows form of b200gate_torch_apply_masks -- apply the masks of the last b200gate_run_rows on this
+ * handle to another set of rows with the same n, row by row (analysis of `in`, the stored masks, synthesis), i.e. the
+ * backward pass of TorchGate.forward(x, lengths=...).  B200GATE_ERR_STATE when the last run was not a rows run, its
+ * masks did not fit one workspace batch, or the row count or an n differs. */
+int b200gate_torch_apply_masks_rows(b200gate_handle* h, const b200gate_row* rows, int64_t n_rows, int dtype, int is_device,
+                                    void* cuda_stream);
 
 /* Sub-range processing for the next b200gate_run calls (SpectralGate.get_traces(start_frame, end_frame),
  * base.py:167-226).  mode 0: the whole recording (default).  mode 1: only chunks [a, b] of the chunk grid

@@ -38,6 +38,7 @@ EXPORTS = [
     "b200gate_host_alloc", "b200gate_host_free",
     "b200gate_stream_begin", "b200gate_stream_push", "b200gate_stream_finish", "b200gate_convert",
     "b200gate_mask_store_bytes", "b200gate_set_mask_store", "b200gate_adjoint", "b200gate_run_rows",
+    "b200gate_torch_apply_masks_rows",
 ]
 
 
@@ -137,6 +138,7 @@ class GateLibrary:
         d.b200gate_set_mask_store.argtypes = [vp, vp, i64]
         d.b200gate_adjoint.argtypes = [vp, vp, vp, vp, C.c_int, i64, i64, i64, i64, C.c_int, vp]
         d.b200gate_run_rows.argtypes = [vp, C.POINTER(Row), i64, C.c_int, C.c_int, vp]
+        d.b200gate_torch_apply_masks_rows.argtypes = [vp, C.POINTER(Row), i64, C.c_int, C.c_int, vp]
 
 
 def format_code(dt) -> int:
@@ -345,6 +347,12 @@ class Gate:
     def torch_apply_masks_device(self, in_ptr, out_ptr, dtype, C_, N, in_stride, out_stride, stream=None):
         self._check(self.lib.dll.b200gate_torch_apply_masks(
             self._h, in_ptr, out_ptr, dtype_code(dtype), C_, N, in_stride, out_stride, 1, stream))
+
+    def torch_apply_masks_rows(self, rows, dtype, is_device, stream=None):
+        """b200gate_torch_apply_masks_rows on (in_ptr, out_ptr, n, channels) tuples: the masks of the last run_rows."""
+        arr = (Row * len(rows))(*rows)
+        self._check(self.lib.dll.b200gate_torch_apply_masks_rows(self._h, arr, len(rows), dtype_code(dtype),
+                                                                 1 if is_device else 0, stream))
 
     # -- kept masks and the adjoint (numpy surface) ---------------------------------------------------------------------
     def mask_store_bytes(self, C_, N) -> int:

@@ -89,6 +89,7 @@ struct b200gate_handle {
     // with the same masks, TorchGate.backward) can reuse them -- b200gate_torch_apply_masks
     bool masks_valid = false, reuse_masks = false;
     long long masks_C = 0, masks_N = 0;
+    std::vector<long long> masks_rows_n;           // ... of a b200gate_run_rows forward: its rows' lengths (else empty)
     // numpy surface: b200gate_set_mask_store's caller-owned buffer.  While it is set, b200gate_run carves the buffers
     // its kernels write the final masks to from it (every unit of the call) instead of from the workspace, and records
     // which run the store holds, so that b200gate_adjoint can check it is handed masks of its own geometry.
@@ -740,7 +741,7 @@ static void launch_stationary_numerators(const b200gate_handle* h, const SmoothA
         }
     } else {
         const int tiles = (tf_hi - tf_lo + sa.TT - 1) / sa.TT;
-        B200_LAUNCH(k_smooth_generic, dim3(tiles, nu), dim3(256), smooth_smem_bytes(sa.TT, nf, nt), st, sa);
+        B200_LAUNCH(k_smooth_generic<>, dim3(tiles, nu), dim3(256), smooth_smem_bytes(sa.TT, nf, nt), st, sa);
     }
 }
 
@@ -1015,11 +1016,15 @@ int b200gate_create(const b200gate_params* p, b200gate_handle** out) {
             });
         cudaFuncSetAttribute(k_smooth_stream<true>, cudaFuncAttributeMaxDynamicSharedMemorySize, 200 * 1024);
         for (int nfb = 1; nfb <= 12; ++nfb) smooth_box_dispatch<true>(SmoothFArgs{}, nfb, dim3(1), 0, nullptr, true);
+        // (torch surface, stationary extents beyond the in-synthesis smoothing: numerators from k_smooth_generic)
+        cudaFuncSetAttribute(k_smooth_generic<true>, cudaFuncAttributeMaxDynamicSharedMemorySize, 160 * 1024);
+        cudaFuncSetAttribute(k2c_synthesize<8, kMaskU16, float, true>, cudaFuncAttributeMaxDynamicSharedMemorySize, k2c_smem_bytes<kMaskU16>());
+        cudaFuncSetAttribute(k2c_synthesize<8, kMaskU16Blend, float, true>, cudaFuncAttributeMaxDynamicSharedMemorySize, k2c_smem_bytes<kMaskU16Blend>());
         cudaFuncSetAttribute(k1n_magnitude_2k, cudaFuncAttributeMaxDynamicSharedMemorySize, k1n2_smem_floats() * 4);
         cudaFuncSetAttribute(k2_synthesize_2k<>, cudaFuncAttributeMaxDynamicSharedMemorySize, k22_smem_floats() * 4);
         cudaFuncSetAttribute(k2_synthesize_2k<true>, cudaFuncAttributeMaxDynamicSharedMemorySize, k22_smem_floats() * 4);
         cudaFuncSetAttribute(k2c_synthesize_2k, cudaFuncAttributeMaxDynamicSharedMemorySize, k2c2_smem_bytes());
-        cudaFuncSetAttribute(k_smooth_generic, cudaFuncAttributeMaxDynamicSharedMemorySize, 160 * 1024);
+        cudaFuncSetAttribute(k_smooth_generic<>, cudaFuncAttributeMaxDynamicSharedMemorySize, 160 * 1024);
         for (int dt = 0; dt < 3; ++dt)
             B200_WITH_DTYPE(dt, { cudaFuncSetAttribute(gk_stft<T>, cudaFuncAttributeMaxDynamicSharedMemorySize, 8192 * 16); });
         cudaFuncSetAttribute(gk_istft, cudaFuncAttributeMaxDynamicSharedMemorySize, 8192 * 16);
@@ -1366,7 +1371,7 @@ int b200gate_torch_set_noise(b200gate_handle* h, const void* xn, int dtype, int6
     TStatArgs ta{};
     ta.n_units = (int)Bn; ta.T = g.T; ta.in_scale = (float)h->sum_w; ta.eps = (float)kEps64; ta.top_db = (float)h->p.top_db;
     ta.n_std = (float)h->p.n_std_thresh; ta.ddof = h->p.std_ddof; ta.mag = mag; ta.rowmax = rowmax; ta.thr = h->d_tthr;
-    B200_LAUNCH(k_tgate_stats, dim3((unsigned)(Bn * kFW)), dim3(kTgWarps * 32), 0, st, ta);
+    B200_LAUNCH(k_tgate_stats<>, dim3((unsigned)(Bn * kFW)), dim3(kTgWarps * 32), 0, st, ta);
     CK(h, cudaGetLastError());
     CK(h, cudaStreamSynchronize(st));
     h->tthr_units = (int)Bn;
@@ -1949,7 +1954,7 @@ static int run_core(b200gate_handle* h, const void* in, void* out, int dtype, in
                 ta.n_units = nu; ta.T = g.T; ta.in_scale = (float)h->sum_w; ta.eps = (float)kEps64;
                 ta.top_db = (float)p.top_db; ta.n_std = (float)p.n_std_thresh; ta.ddof = p.std_ddof;
                 ta.mag = d_tdb; ta.rowmax = d_trow; ta.thr = d_tthr_self;
-                B200_LAUNCH(k_tgate_stats, dim3((unsigned)((long long)nu * kFW)), dim3(kTgWarps * 32), 0, st, ta);
+                B200_LAUNCH(k_tgate_stats<>, dim3((unsigned)((long long)nu * kFW)), dim3(kTgWarps * 32), 0, st, ta);
                 TBitsArgs ba{};
                 ba.n_units = nu; ba.T = g.T; ba.top_db = (float)p.top_db; ba.db = d_tdb; ba.rowmax = d_trow; ba.bits = d_bits;
                 if (h->tthr_units > 0) {
@@ -1959,7 +1964,7 @@ static int run_core(b200gate_handle* h, const void* in, void* out, int dtype, in
                     ba.thr = d_tthr_self;
                     ba.thr_units = nu;
                 }
-                B200_LAUNCH(k_tgate_bits, dim3((unsigned)((long long)nu * kFW)), dim3(kTgWarps * 32), 0, st, ba);
+                B200_LAUNCH(k_tgate_bits<>, dim3((unsigned)((long long)nu * kFW)), dim3(kTgWarps * 32), 0, st, ba);
                 CK(h, cudaMemsetAsync(d_rowflag, 0, (size_t)nu * kFW * 4, st));
                 ++launches;
                 }
@@ -2184,7 +2189,7 @@ static int run_core(b200gate_handle* h, const void* in, void* out, int dtype, in
                     TMovArgs ma{};
                     ma.n_units = nu; ma.T = g.T; ma.n_movemean = p.n_movemean; ma.n_thresh = (float)p.thresh_n_mult;
                     ma.inv_temp = (float)p.sigmoid_slope; ma.p = (float)p.prop_decrease; ma.mag = d_mag; ma.m0 = d_m0;
-                    B200_LAUNCH(k_tgate_movmean, dim3(grid_1d((long long)nu * kFPad, 128, 1 << 30)), dim3(128), 0, st, ma);
+                    B200_LAUNCH(k_tgate_movmean<>, dim3(grid_1d((long long)nu * kFPad, 128, 1 << 30)), dim3(128), 0, st, ma);
                 } else {
                     IirArgs ia{};
                     ia.n_units = nu; ia.T = g.T; ia.F = kF; ia.FPad = kFPad;
@@ -2342,6 +2347,7 @@ static int run_core(b200gate_handle* h, const void* in, void* out, int dtype, in
     h->stats_pending = true;
     if (torch_sem && !generic && !two_k && n_batches == 1 && !h->reuse_masks) {
         h->masks_valid = true; h->masks_C = C; h->masks_N = N;
+        h->masks_rows_n.clear();
     }
     h->pend_batches = n_batches;
     if (keep) {
@@ -2376,22 +2382,37 @@ int b200gate_run_rows(b200gate_handle* h, const b200gate_row* rows, int64_t n_ro
     if (!h || !rows || n_rows <= 0 || dtype_size(dtype) == 0) return fail(h, B200GATE_ERR_ARG, "bad argument");
     if (h->s_open) return fail(h, B200GATE_ERR_STATE, "a stream is open on this handle (b200gate_stream_finish first)");
     const b200gate_params& p = h->p;
-    if (p.surface != B200GATE_SURFACE_NUMPY) return fail(h, B200GATE_ERR_STATE, "b200gate_run_rows is for the numpy surface");
+    // torch: TorchGate.forward on each row (one unit per row: no chunk grid, no padding, torch.istft output length)
+    const bool torch = p.surface == B200GATE_SURFACE_TORCH;
+    if (p.surface != B200GATE_SURFACE_NUMPY && !torch)
+        return fail(h, B200GATE_ERR_STATE, "b200gate_run_rows is for the numpy and torch surfaces");
     if (h->mask_store) return fail(h, B200GATE_ERR_STATE, "b200gate_run_rows keeps no masks (b200gate_set_mask_store(NULL) first)");
     if (h->range_mode != 0) return fail(h, B200GATE_ERR_STATE, "b200gate_run_rows runs whole rows (b200gate_set_range(0) first)");
-    if (h->generic || p.n_fft != kN) return fail(h, B200GATE_ERR_ARG, "b200gate_run_rows needs n_fft = win_length = 1024, hop_length = 256");
+    if (h->generic || p.n_fft != kN)                            // (a big smoothing filter also makes the handle generic)
+        return fail(h, B200GATE_ERR_ARG, "b200gate_run_rows runs the n_fft 1024 kernels: it needs n_fft = win_length = 1024, "
+                    "hop_length = 256 and smoothing extents (%d, %d) within their 16-bit numerators ((nf + 1)^2 (nt + 1)^2 "
+                    "<= 65535, at most 64 a side)", p.n_grad_freq, p.n_grad_time);
     if (p.path_flags != 0) return fail(h, B200GATE_ERR_ARG, "b200gate_run_rows runs the default kernel selection (path_flags = 0)");
+    if (torch && dtype != B200GATE_F32) return fail(h, B200GATE_ERR_ARG, "b200gate_run_rows: the torch surface runs float32 rows");
     const bool stat = p.stationary != 0;
     const int nf = p.n_grad_freq, nt = p.n_grad_time;
-    if (stat && !packed_smoothing_fits(nf, nt))
+    // stationary: smoothing in the synthesis kernel where the byte lanes hold the filter; on the torch surface the
+    // numerator kernel k_smooth_generic takes the other extents
+    const bool smooth_in_k2 = packed_smoothing_fits(nf, nt);
+    if (stat && !torch && !smooth_in_k2)
         return fail(h, B200GATE_ERR_ARG, "b200gate_run_rows: stationary smoothing extents (%d, %d) beyond the in-synthesis smoothing", nf, nt);
     if (!stat && !((nf >= 1 && nf <= 12 && smoothb_smem_bytes(kFPad, nt) <= 200 * 1024) || smooths_smem_bytes(kFPad, nf, nt) <= 200 * 1024))
         return fail(h, B200GATE_ERR_ARG, "b200gate_run_rows: smoothing extents (%d, %d) beyond the streaming smoothing kernels", nf, nt);
-    if (stat && !h->have_thresh) return fail(h, B200GATE_ERR_STATE, "stationary gate: call b200gate_noise_stats first");
+    if (stat && !torch && !h->have_thresh) return fail(h, B200GATE_ERR_STATE, "stationary gate: call b200gate_noise_stats first");
+    if (torch && h->tthr_units > 1 && h->tthr_units != n_rows)
+        return fail(h, B200GATE_ERR_ARG, "xn has %d rows, the call has %lld", h->tthr_units, (long long)n_rows);
     cudaStream_t st = (cudaStream_t)stream;
     const size_t es = dtype_size(dtype);
     const int H = p.hop_length;
-    const long long pad = p.padding, cs = p.chunk_size;
+    const long long pad = torch ? 0 : p.padding, cs = torch ? 0 : p.chunk_size;
+    const bool reuse = h->reuse_masks;                          // b200gate_torch_apply_masks_rows
+    // torch.istft(center=True) length of an n-sample row (torchgate.py:255-262)
+    auto out_len = [&](long long n) { return torch ? (n / H) * H + (p.n_fft & 1) : n; };
 
     // ---- the unit table -------------------------------------------------------------------------------------
     const char *in_lo = nullptr, *in_hi = nullptr, *out_lo = nullptr, *out_hi = nullptr;    // spans covering the rows
@@ -2401,16 +2422,18 @@ int b200gate_run_rows(b200gate_handle* h, const b200gate_row* rows, int64_t n_ro
         const b200gate_row& rw = rows[r];
         if (!rw.in || !rw.out || rw.n <= 0 || rw.channels <= 0)
             return fail(h, B200GATE_ERR_ARG, "row %lld: null pointer, no samples or no channels", (long long)r);
+        if (torch && rw.n < 2 * p.win_length)
+            return fail(h, B200GATE_ERR_ARG, "row %lld: x must be bigger than %d", (long long)r, 2 * p.win_length);
         const char *a = (const char*)rw.in, *b = (const char*)rw.out;
-        const size_t nb = (size_t)rw.n * es;
-        if (a < b + nb && b < a + nb) return fail(h, B200GATE_ERR_ARG, "row %lld: out aliases in", (long long)r);
+        const size_t nb = (size_t)rw.n * es, nbo = (size_t)out_len(rw.n) * es;
+        if (a < b + nbo && b < a + nb) return fail(h, B200GATE_ERR_ARG, "row %lld: out aliases in", (long long)r);
         const long long Lp = (cs > 0 && rw.n > cs ? cs : rw.n) + 2 * pad;
         if (Lp / H > 0x3fffffffLL) return fail(h, B200GATE_ERR_ARG, "problem too large");
         U += cs > 0 && rw.n > cs ? (rw.n - 1) / cs + 1 : 1;
         if (!in_lo || a < in_lo) in_lo = a;
         if (!in_hi || a + nb > in_hi) in_hi = a + nb;
         if (!out_lo || b < out_lo) out_lo = b;
-        if (!out_hi || b + nb > out_hi) out_hi = b + nb;
+        if (!out_hi || b + nbo > out_hi) out_hi = b + nbo;
         row_bytes += nb;
     }
     if (U > 0x7fffffffLL) return fail(h, B200GATE_ERR_ARG, "problem too large");
@@ -2471,8 +2494,9 @@ int b200gate_run_rows(b200gate_handle* h, const b200gate_row* rows, int64_t n_ro
                     h_hi = (int)((jp_hi + kN / 2 + H - 1) / H);
                     d.tf_hi = std::min(h_hi, d.T);
                 }
-                d.regen = stat ? 0 : iir_regen_ok(b_iir, d.T, 0);
-                if (pad + step > sig_len) zero_units.push_back(u);               // stationary.py:126 leaves the tail zero
+                d.regen = stat || torch ? 0 : iir_regen_ok(b_iir, d.T, 0);
+                // stationary.py:126 leaves the tail zero (a torch row's output ends with its istft length)
+                if (!torch && pad + step > sig_len) zero_units.push_back(u);
                 {   // hops per synthesis work item: run_core's choice for a [channels][n] recording in one workspace batch
                     const long long hops = std::max(0, h_hi - h_lo), want = (long long)resident * kWarps * 4;
                     long long run = std::max(16LL, std::min(128LL, (nch * rw.channels * hops + want - 1) / want));
@@ -2487,12 +2511,13 @@ int b200gate_run_rows(b200gate_handle* h, const b200gate_row* rows, int64_t n_ro
         }
     }
     h->stats = b200gate_stats{};
-    h->masks_valid = false;
+    if (!reuse) h->masks_valid = false;
     long long launches = 0;
     CK(h, cudaMemcpyAsync(h->d_units, h->hp_units, tbytes, cudaMemcpyHostToDevice, st));
     CK(h, cudaEventRecord(h->ev_units, st));
     const UnitDesc* d_units = (const UnitDesc*)h->d_units;
     if (!is_device) CK(h, cudaMemcpyAsync(h->d_in, in_lo, in_span, cudaMemcpyHostToDevice, st));
+    if (!is_device && torch) CK(h, cudaMemsetAsync(h->d_out, 0, out_span, st));     // (the span's bytes between rows)
     for (long long u : zero_units) {
         const UnitDesc& d = h->hp_units[u];
         CK(h, cudaMemsetAsync((char*)d.y + (size_t)d.o_lo * es, 0, (size_t)(d.o_hi - d.o_lo) * es, st));
@@ -2503,8 +2528,12 @@ int b200gate_run_rows(b200gate_handle* h, const b200gate_row* rows, int64_t n_ro
     g.H = H; g.C = 1; g.T = T_max; g.pad = pad;
     const int zpairs = (T_max + 1) / 2;
     const size_t zunit = (size_t)zpairs * 1024 * sizeof(float2);
+    // torch surface, stationary: the dB spectrogram, its row maxima and self thresholds, and the numerators of
+    // k_smooth_generic when the synthesis kernel cannot smooth the decisions itself
+    const size_t num_bytes = smooth_in_k2 ? 0 : (size_t)num_unit_stride(T_max) * 2;
     const size_t per_unit = (stat ? (size_t)T_max * kFW * 4 + (size_t)kFPad * 4 + (size_t)kFW * 4 + 64
-                                  : 2 * (size_t)T_max * kFPad * 4 + 64) + 2048 + zunit;
+                                  : 2 * (size_t)T_max * kFPad * 4 + 64) +
+                            (stat && torch ? num_bytes + (size_t)T_max * kFPad * 4 + 2 * (size_t)kFPad * 4 : 0) + 2048 + zunit;
     double limit = p.workspace_limit_bytes;
     if (!(limit > 0)) {
         limit = 24.0 * 1024 * 1024 * 1024;
@@ -2512,7 +2541,8 @@ int b200gate_run_rows(b200gate_handle* h, const b200gate_row* rows, int64_t n_ro
         if (cudaMemGetInfo(&free_b, &total_b) == cudaSuccess)
             limit = std::min(limit, 0.7 * ((double)free_b + (double)h->ws_bytes));
     }
-    long long ub = std::min(U, (long long)std::max(1.0, floor(limit / (double)per_unit)));
+    // the backward applies the masks the forward left in its one workspace batch: same units, same layout
+    long long ub = reuse ? U : std::min(U, (long long)std::max(1.0, floor(limit / (double)per_unit)));
     for (;;) {                                                  // as run_core: halve the batch if the device cannot give it
         if (ensure(h, (void**)&h->d_ws_buf, &h->ws_bytes, (size_t)ub * per_unit + ((size_t)8 << 20)) == B200GATE_OK) break;
         cudaGetLastError();
@@ -2526,7 +2556,11 @@ int b200gate_run_rows(b200gate_handle* h, const b200gate_row* rows, int64_t n_ro
     auto al = [](size_t v) { return (v + 255) / 256 * 256; };
     const size_t off_rowmax = al((size_t)ub * T_max * kFW * 4);
     const size_t off_rowflag = off_rowmax + al((size_t)ub * kFPad * 4);
-    const size_t end_stat = off_rowflag + al((size_t)ub * kFW * 4);
+    const size_t off_num = off_rowflag + al((size_t)ub * kFW * 4);
+    const size_t off_tdb = off_num + al((size_t)ub * num_bytes);
+    const size_t off_trow = off_tdb + al((size_t)ub * T_max * kFPad * 4);
+    const size_t off_tthr = off_trow + al((size_t)ub * kFPad * 4);
+    const size_t end_stat = torch ? off_tthr + al((size_t)ub * kFPad * 4) : off_num;
     const size_t off_m0 = al((size_t)ub * T_max * kFPad * 4);
     const size_t end_nonstat = off_m0 + al((size_t)ub * T_max * kFPad * 4);
     const size_t off_z = al(stat ? end_stat : end_nonstat);
@@ -2537,6 +2571,10 @@ int b200gate_run_rows(b200gate_handle* h, const b200gate_row* rows, int64_t n_ro
     unsigned* d_bits = (unsigned*)h->d_ws_buf;
     unsigned* d_rowmax = (unsigned*)(h->d_ws_buf + off_rowmax);
     unsigned* d_rowflag = (unsigned*)(h->d_ws_buf + off_rowflag);
+    unsigned short* d_num = (unsigned short*)(h->d_ws_buf + off_num);
+    float* d_tdb = (float*)(h->d_ws_buf + off_tdb);
+    float* d_trow = (float*)(h->d_ws_buf + off_trow);
+    float* d_tthr_self = (float*)(h->d_ws_buf + off_tthr);
     float* d_mag = (float*)h->d_ws_buf;
     float* d_m0 = (float*)(h->d_ws_buf + off_m0);
     float2* d_zcache = (float2*)(h->d_ws_buf + off_z);
@@ -2570,7 +2608,68 @@ int b200gate_run_rows(b200gate_handle* h, const b200gate_row* rows, int64_t n_ro
         a2.n_runs = (int)n_runs2;
         const unsigned grid2 = (unsigned)grid_1d((long long)nu * a2.n_runs, kWarps, resident);
         cudaEventRecord(h->stage_ev[4 * bi + 0], st);
-        if (stat) {
+        K1nArgs an{};                                           // k1n_magnitude: the torch surface and the non-stationary gate
+        an.g = g; an.tb = tb; an.dbg = dbg; an.zcache = d_zcache; an.zpairs = zpairs;
+        an.z_lo = tf_lo; an.z_hi = tf_hi_max + 1; an.units = d_units;
+        an.run = (int)run1; an.n_runs = n_runs1;
+        const unsigned grid1n = (unsigned)grid_1d((long long)nu * n_runs1, kWarps, resident);
+        if (stat && torch) {
+            // TorchGate (run_core): |X| -> dB, statistics over each row's own frames (or xn's), compare; the backward
+            // (reuse) re-transforms only and synthesises with the decisions / numerators the forward left in the workspace
+            an.mag = reuse ? nullptr : d_tdb;
+            { auto kern_ = k1n_magnitude<8, float, true>;
+              B200_LAUNCH(kern_, dim3(grid1n), dim3(kThreads), k1n_smem_floats() * 4, st, an); }
+            ++launches;
+            if (!reuse) {
+                TStatArgs ta{};
+                ta.n_units = nu; ta.T = T_max; ta.in_scale = (float)h->sum_w; ta.eps = (float)kEps64;
+                ta.top_db = (float)p.top_db; ta.n_std = (float)p.n_std_thresh; ta.ddof = p.std_ddof;
+                ta.mag = d_tdb; ta.rowmax = d_trow; ta.thr = d_tthr_self; ta.units = d_units + u0;
+                { auto kern_ = k_tgate_stats<true>;
+                  B200_LAUNCH(kern_, dim3((unsigned)((long long)nu * kFW)), dim3(kTgWarps * 32), 0, st, ta); }
+                TBitsArgs ba{};
+                ba.n_units = nu; ba.T = T_max; ba.top_db = (float)p.top_db; ba.db = d_tdb; ba.rowmax = d_trow; ba.bits = d_bits;
+                ba.units = d_units + u0;
+                if (h->tthr_units > 0) {                        // xn: one row for every unit, or row r for unit r
+                    ba.thr = h->tthr_units == 1 ? h->d_tthr : h->d_tthr + (size_t)u0 * kFPad;
+                    ba.thr_units = h->tthr_units == 1 ? 1 : nu;
+                } else {
+                    ba.thr = d_tthr_self;
+                    ba.thr_units = nu;
+                }
+                { auto kern_ = k_tgate_bits<true>;
+                  B200_LAUNCH(kern_, dim3((unsigned)((long long)nu * kFW)), dim3(kTgWarps * 32), 0, st, ba); }
+                CK(h, cudaMemsetAsync(d_rowflag, 0, (size_t)nu * kFW * 4, st));
+                launches += 2;
+                if (!smooth_in_k2 && tf_hi_max > tf_lo) {
+                    SmoothArgs sa{};
+                    sa.n_units = nu; sa.T = T_max; sa.nf = nf; sa.nt = nt; sa.tf_lo = tf_lo; sa.tf_hi = tf_hi_max; sa.TT = 32;
+                    sa.bits = d_bits; sa.rowflag = d_rowflag; sa.num = d_num; sa.units = d_units + u0;
+                    auto kern_ = k_smooth_generic<true>;
+                    B200_LAUNCH(kern_, dim3((tf_hi_max - tf_lo + sa.TT - 1) / sa.TT, nu), dim3(256),
+                                smooth_smem_bytes(sa.TT, nf, nt), st, sa);
+                    ++launches;
+                }
+            }
+            cudaEventRecord(h->stage_ev[4 * bi + 1], st);
+            cudaEventRecord(h->stage_ev[4 * bi + 2], st);
+            if (hops > 0) {
+                a2.pD = (float)(p.prop_decrease / D);
+                a2.one_minus_p = (float)(1.0 - p.prop_decrease);
+                const bool blend = a2.one_minus_p != 0.f;
+                if (smooth_in_k2) {
+                    a2.bits = d_bits; a2.rowflag = d_rowflag;
+                    set_k2c_smoothing_taps(a2, nf);
+                    auto kern2 = blend ? k2c_synthesize<8, kMaskBitsBlend, float, true> : k2c_synthesize<8, kMaskBits, float, true>;
+                    B200_LAUNCH(kern2, dim3(grid2), dim3(kThreads), k2c_smem_bytes<kMaskBits>(), st, a2);
+                } else {
+                    a2.num = d_num;
+                    auto kern2 = blend ? k2c_synthesize<8, kMaskU16Blend, float, true> : k2c_synthesize<8, kMaskU16, float, true>;
+                    B200_LAUNCH(kern2, dim3(grid2), dim3(kThreads), k2c_smem_bytes<kMaskU16>(), st, a2);
+                }
+                ++launches;
+            }
+        } else if (stat) {
             CK(h, cudaMemsetAsync(d_rowmax, 0, (size_t)nu * kFPad * 4, st));
             CK(h, cudaMemsetAsync(h->d_need_rowmax, 0, sizeof(unsigned), st));
             K1Args a1{};
@@ -2606,26 +2705,34 @@ int b200gate_run_rows(b200gate_handle* h, const b200gate_row* rows, int64_t n_ro
                 ++launches;
             }
         } else {
-            K1nArgs a1{};
-            a1.g = g; a1.tb = tb; a1.mag = d_mag; a1.dbg = dbg; a1.zcache = d_zcache; a1.zpairs = zpairs;
-            a1.z_lo = tf_lo; a1.z_hi = tf_hi_max + 1; a1.units = d_units;
-            a1.run = (int)run1; a1.n_runs = n_runs1;
+            an.mag = reuse ? nullptr : d_mag;
             B200_WITH_DTYPE(dtype, { auto kern_ = k1n_magnitude<8, T, true>;
-                B200_LAUNCH(kern_, dim3(grid_1d((long long)nu * n_runs1, kWarps, resident)), dim3(kThreads),
-                            k1n_smem_floats() * 4, st, a1); });
+                B200_LAUNCH(kern_, dim3(grid1n), dim3(kThreads), k1n_smem_floats() * 4, st, an); });
             cudaEventRecord(h->stage_ev[4 * bi + 1], st);
-            IirArgs ia{};
-            ia.n_units = nu; ia.T = T_max; ia.F = kF; ia.FPad = kFPad; ia.b = b_iir;
-            ia.n_mult = (float)p.thresh_n_mult; ia.slope = (float)p.sigmoid_slope;
-            ia.mag = d_mag; ia.m0 = d_m0; ia.units = d_units + u0;    // (regen: each unit's own, UnitDesc::regen)
-            { auto kern_ = k_iir_sigmoid<kFPad, true>;
-              B200_LAUNCH(kern_, dim3(grid_1d((long long)nu * kFPad, 128, 1 << 30)), dim3(128), 0, st, ia); }
-            launches += 2;
-            if (tf_hi_max > tf_lo) {
+            if (reuse) {
+                // the final masks of the forward are still in d_mag
+            } else if (torch) {                                 // torchgate.py:168-198: moving-mean follower
+                TMovArgs ma{};
+                ma.n_units = nu; ma.T = T_max; ma.n_movemean = p.n_movemean; ma.n_thresh = (float)p.thresh_n_mult;
+                ma.inv_temp = (float)p.sigmoid_slope; ma.p = (float)p.prop_decrease; ma.mag = d_mag; ma.m0 = d_m0;
+                ma.units = d_units + u0;
+                auto kern_ = k_tgate_movmean<true>;
+                B200_LAUNCH(kern_, dim3(grid_1d((long long)nu * kFPad, 128, 1 << 30)), dim3(128), 0, st, ma);
+            } else {
+                IirArgs ia{};
+                ia.n_units = nu; ia.T = T_max; ia.F = kF; ia.FPad = kFPad; ia.b = b_iir;
+                ia.n_mult = (float)p.thresh_n_mult; ia.slope = (float)p.sigmoid_slope;
+                ia.mag = d_mag; ia.m0 = d_m0; ia.units = d_units + u0;    // (regen: each unit's own, UnitDesc::regen)
+                { auto kern_ = k_iir_sigmoid<kFPad, true>;
+                  B200_LAUNCH(kern_, dim3(grid_1d((long long)nu * kFPad, 128, 1 << 30)), dim3(128), 0, st, ia); }
+            }
+            launches += reuse ? 1 : 2;
+            if (tf_hi_max > tf_lo && !reuse) {
                 SmoothFArgs sa{};
                 sa.n_units = nu; sa.T = T_max; sa.nf = nf; sa.nt = nt; sa.tf_lo = tf_lo; sa.tf_hi = tf_hi_max; sa.TT = 32;
                 sa.F = kF; sa.FPad = kFPad;
-                sa.p = (float)p.prop_decrease; sa.one_minus_p = (float)(1.0 - p.prop_decrease);
+                // the torch surface blends before the smoothing (in k_tgate_movmean, torchgate.py:241)
+                sa.p = torch ? 1.0f : (float)p.prop_decrease; sa.one_minus_p = torch ? 0.0f : (float)(1.0 - p.prop_decrease);
                 sa.m0 = d_m0; sa.m2 = d_mag; sa.units = d_units + u0;
                 launch_smooth_float<true>(sa, nf, nt, tf_lo, tf_hi_max, nu, 0, st);      // (extents checked on entry)
                 ++launches;
@@ -2650,6 +2757,11 @@ int b200gate_run_rows(b200gate_handle* h, const b200gate_row* rows, int64_t n_ro
     h->stats.kernel_launches = launches;
     h->stats_pending = true;
     h->pend_batches = n_batches;
+    if (torch && n_batches == 1 && !reuse) {      // the masks stay in the workspace for b200gate_torch_apply_masks_rows
+        h->masks_valid = true; h->masks_C = 0; h->masks_N = 0;
+        h->masks_rows_n.resize((size_t)n_rows);
+        for (int64_t r = 0; r < n_rows; ++r) h->masks_rows_n[(size_t)r] = rows[r].n;
+    }
     if (!is_device) {                            // host rows: the results must be in place on return
         const int rc = resolve_stats(h);
         if (rc) return rc;
@@ -3066,6 +3178,22 @@ int b200gate_torch_apply_masks(b200gate_handle* h, const void* in, void* out, in
                     "tuned n_fft=1024 geometry, one workspace batch)", (long long)C, (long long)N);
     h->reuse_masks = true;
     const int rc = b200gate_run(h, in, out, dtype, C, N, in_stride, out_stride, is_device, stream);
+    h->reuse_masks = false;
+    return rc;
+}
+
+int b200gate_torch_apply_masks_rows(b200gate_handle* h, const b200gate_row* rows, int64_t n_rows, int dtype, int is_device,
+                                    void* stream) {
+    if (!h) return B200GATE_ERR_ARG;
+    if (h->p.surface != B200GATE_SURFACE_TORCH) return fail(h, B200GATE_ERR_STATE, "torch surface only");
+    if (!rows || n_rows <= 0) return fail(h, B200GATE_ERR_ARG, "bad argument");
+    bool match = h->masks_valid && (int64_t)h->masks_rows_n.size() == n_rows;
+    for (int64_t r = 0; match && r < n_rows; ++r) match = rows[r].n == h->masks_rows_n[(size_t)r];
+    if (!match)
+        return fail(h, B200GATE_ERR_STATE, "no masks of a matching forward are kept (run b200gate_run_rows on %lld rows of the "
+                    "same lengths first; one workspace batch)", (long long)n_rows);
+    h->reuse_masks = true;
+    const int rc = b200gate_run_rows(h, rows, n_rows, dtype, is_device, stream);
     h->reuse_masks = false;
     return rc;
 }

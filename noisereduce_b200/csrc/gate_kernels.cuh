@@ -672,6 +672,8 @@ struct SmoothArgs {
     const unsigned* bits;      // [n_units][T][FW]
     const unsigned* rowflag;   // [n_units][FW]
     unsigned short* num;       // [n_units][ceil(T/2)][FPad][2]  (num_index)
+    const UnitDesc* units;     // ROWS instantiations: units + (first unit of the batch); T is then the pitch only and
+                               // tf_hi the largest of the batch
 };
 
 __host__ __device__ inline int smooth_rows(int TT, int nt) { return TT + 2 * nt + 2 * (nt + 1); }
@@ -680,6 +682,7 @@ inline size_t smooth_smem_bytes(int TT, int nf, int nt) {
     return (size_t)smooth_rows(TT, nt) * kFW * 4 + (size_t)TT * smooth_cpitch(nf) * 2 + 16;
 }
 
+template <bool ROWS = false>
 __global__ void __launch_bounds__(256) k_smooth_generic(const SmoothArgs a) {
     B200_DYN_SMEM(unsigned, smem);
     const int nt = a.nt, nf = a.nf, aa = nt + 1;
@@ -688,16 +691,17 @@ __global__ void __launch_bounds__(256) k_smooth_generic(const SmoothArgs a) {
     unsigned* s_bits = smem;                                                   // [rows][FW]
     unsigned short* s_c = reinterpret_cast<unsigned short*>(smem + rows * kFW);  // [TT][cp]
     const int ul = blockIdx.y;
+    const int T = ROWS ? a.units[ul].T : a.T, tf_hi = ROWS ? a.units[ul].tf_hi : a.tf_hi;
     const int t0 = a.tf_lo + blockIdx.x * a.TT;
-    if (t0 >= a.tf_hi) return;
-    const int tt_n = min(a.TT, a.tf_hi - t0);
+    if (t0 >= tf_hi) return;
+    const int tt_n = min(a.TT, tf_hi - t0);
     // row rho <-> frame tau = t0 - nt - 2aa + rho ; the first 2aa rows are "before the stream" = 0
     const int tau0 = t0 - nt - 2 * aa;
     for (int i = threadIdx.x; i < rows * kFW; i += blockDim.x) {
         const int rho = i / kFW, w = i - rho * kFW;
         const int tau = tau0 + rho;
         unsigned v = 0u;
-        if (rho >= 2 * aa && tau >= 0 && tau < a.T)
+        if (rho >= 2 * aa && tau >= 0 && tau < T)
             v = a.bits[((long long)ul * a.T + tau) * kFW + w] | a.rowflag[ul * kFW + w];
         s_bits[i] = v;
     }
@@ -1702,6 +1706,7 @@ struct TStatArgs {
     float* mag;                // in: |X| / sum(w);  out: dB (float32), unclamped
     float* rowmax;             // [n_units][FPad] max_t dB
     float* thr;                // [n_units][FPad] mean + n_std * std of the clamped dB
+    const UnitDesc* units;     // ROWS instantiations: units + (first unit of the batch); T is then the pitch only
 };
 
 // One CTA per (unit, 32-bin group); its kTgWarps warps share the frames (warp w takes t = w, w + kTgWarps, ...), every access
@@ -1710,11 +1715,13 @@ struct TStatArgs {
 // a 256-row batch with 139 k threads and the column walks latency-bound (0.38 + 0.29 ms of a 1.47 ms forward).
 constexpr int kTgWarps = 8;
 
+template <bool ROWS = false>
 __global__ void __launch_bounds__(kTgWarps * 32) k_tgate_stats(const TStatArgs a) {
     __shared__ double s_red[kTgWarps][32];
     __shared__ float s_mx[kTgWarps][32];
     const int lane = threadIdx.x & 31, w = threadIdx.x >> 5;
     const int ul = blockIdx.x / kFW, grp = blockIdx.x - ul * kFW;
+    const int T = ROWS ? a.units[ul].T : a.T;             // ROWS: the unit's own frames
     const int f = grp * 32 + lane;
     const long long idx = (long long)ul * kFPad + f;
     float* D = a.mag + (long long)ul * a.T * kFPad + f;
@@ -1722,7 +1729,7 @@ __global__ void __launch_bounds__(kTgWarps * 32) k_tgate_stats(const TStatArgs a
     float mx = -INFINITY;
     if (live) {
 #pragma unroll 4
-        for (int t = w; t < a.T; t += kTgWarps) {
+        for (int t = w; t < T; t += kTgWarps) {
             const float db = 20.0f * log10f(D[(long long)t * kFPad] * a.in_scale + a.eps);
             D[(long long)t * kFPad] = db;
             mx = fmaxf(mx, db);
@@ -1736,19 +1743,19 @@ __global__ void __launch_bounds__(kTgWarps * 32) k_tgate_stats(const TStatArgs a
     double sum = 0.0;
     if (live) {
 #pragma unroll 4
-        for (int t = w; t < a.T; t += kTgWarps) sum += (double)fmaxf(D[(long long)t * kFPad], fl);     // (this thread's own stores)
+        for (int t = w; t < T; t += kTgWarps) sum += (double)fmaxf(D[(long long)t * kFPad], fl);     // (this thread's own stores)
     }
     s_red[w][lane] = sum;
     __syncthreads();
     sum = 0.0;
 #pragma unroll
     for (int k = 0; k < kTgWarps; ++k) sum += s_red[k][lane];
-    const double mean = sum / a.T;
+    const double mean = sum / T;
     __syncthreads();
     double ss = 0.0;
     if (live) {
 #pragma unroll 4
-        for (int t = w; t < a.T; t += kTgWarps) {
+        for (int t = w; t < T; t += kTgWarps) {
             const double d = (double)fmaxf(D[(long long)t * kFPad], fl) - mean;
             ss += d * d;
         }
@@ -1759,7 +1766,7 @@ __global__ void __launch_bounds__(kTgWarps * 32) k_tgate_stats(const TStatArgs a
         ss = 0.0;
 #pragma unroll
         for (int k = 0; k < kTgWarps; ++k) ss += s_red[k][lane];
-        const double sd = sqrt(ss / (double)(a.T - a.ddof));
+        const double sd = sqrt(ss / (double)(T - a.ddof));
         a.rowmax[idx] = live ? mx : -INFINITY;
         a.thr[idx] = live ? (float)(mean + sd * (double)a.n_std) : INFINITY;
     }
@@ -1773,11 +1780,14 @@ struct TBitsArgs {
     const float* rowmax;       // [n_units][FPad]  (of x itself)
     const float* thr;          // [thr_units][FPad]
     unsigned* bits;            // [n_units][T][FW]
+    const UnitDesc* units;     // ROWS instantiations: units + (first unit of the batch); T is then the pitch only
 };
 
+template <bool ROWS = false>
 __global__ void __launch_bounds__(kTgWarps * 32) k_tgate_bits(const TBitsArgs a) {
     const int lane = threadIdx.x & 31, w = threadIdx.x >> 5;
     const int ul = blockIdx.x / kFW, grp = blockIdx.x - ul * kFW;
+    const int T = ROWS ? a.units[ul].T : a.T;             // ROWS: the unit's own frames
     const int f = grp * 32 + lane;
     const float* D = a.db + (long long)ul * a.T * kFPad + f;
     const float fl = a.rowmax[(long long)ul * kFPad + f] - a.top_db;
@@ -1785,18 +1795,18 @@ __global__ void __launch_bounds__(kTgWarps * 32) k_tgate_bits(const TBitsArgs a)
     const bool live = f < kF;
     unsigned* brow = a.bits + (long long)ul * a.T * kFW + grp;
     constexpr int kU = 4;                                   // rows requested together, then voted on
-    for (int t0 = w; t0 < a.T; t0 += kU * kTgWarps) {
+    for (int t0 = w; t0 < T; t0 += kU * kTgWarps) {
         float v[kU];
 #pragma unroll
         for (int j = 0; j < kU; ++j) {
             const int t = t0 + j * kTgWarps;
-            v[j] = (t < a.T) ? D[(long long)t * kFPad] : -INFINITY;
+            v[j] = (t < T) ? D[(long long)t * kFPad] : -INFINITY;
         }
 #pragma unroll
         for (int j = 0; j < kU; ++j) {
             const int t = t0 + j * kTgWarps;
             const unsigned word = __ballot_sync(0xffffffffu, live && (fmaxf(v[j], fl) > th));
-            if (t < a.T && lane == 0) brow[(long long)t * kFW] = word;
+            if (t < T && lane == 0) brow[(long long)t * kFW] = word;
         }
     }
 }
@@ -1807,30 +1817,33 @@ struct TMovArgs {
     float n_thresh, inv_temp, p;
     const float* mag;
     float* m0;                 // blended sigmoid mask, prop_decrease * (m - 1) + 1 (torchgate.py:241)
+    const UnitDesc* units;     // ROWS instantiations: units + (first unit of the batch); T is then the pitch only
 };
 
+template <bool ROWS = false>
 __global__ void __launch_bounds__(128) k_tgate_movmean(const TMovArgs a) {
     const long long idx = (long long)blockIdx.x * blockDim.x + threadIdx.x;
     if (idx >= (long long)a.n_units * kFPad) return;
     const int ul = (int)(idx / kFPad), f = (int)(idx - (long long)ul * kFPad);
+    const int T = ROWS ? a.units[ul].T : a.T;             // ROWS: the unit's own frames (conv1d's "same" edges)
     const float* A = a.mag + (long long)ul * a.T * kFPad + f;
     float* M = a.m0 + (long long)ul * a.T * kFPad + f;
     if (f >= kF) {
-        for (int t = 0; t < a.T; ++t) M[(long long)t * kFPad] = 0.f;
+        for (int t = 0; t < T; ++t) M[(long long)t * kFPad] = 0.f;
         return;
     }
     // conv1d(ones(n), padding="same"): window [t - left, t + right], zero padded, left = (n-1)/2
     const int n = a.n_movemean, left = (n - 1) / 2, right = n - 1 - left;
     double run = 0.0;
-    for (int t = 0; t <= right && t < a.T; ++t) run += (double)A[(long long)t * kFPad];
-    for (int t = 0; t < a.T; ++t) {
+    for (int t = 0; t <= right && t < T; ++t) run += (double)A[(long long)t * kFPad];
+    for (int t = 0; t < T; ++t) {
         const float Av = A[(long long)t * kFPad];
         const float S = (float)(run / (double)n);
         const float r = (Av - S) / S;
         const float m = 1.0f / (1.0f + expf(-(r - a.n_thresh) * a.inv_temp));
         M[(long long)t * kFPad] = a.p * (m - 1.0f) + 1.0f;
         const int tin = t + 1 + right, tout = t - left;
-        if (tin < a.T) run += (double)A[(long long)tin * kFPad];
+        if (tin < T) run += (double)A[(long long)tin * kFPad];
         if (tout >= 0) run -= (double)A[(long long)tout * kFPad];
     }
 }

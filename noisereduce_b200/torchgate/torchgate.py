@@ -99,7 +99,18 @@ class TorchGate(torch.nn.Module):
             self._gate[key] = gate
         return gate
 
-    def forward(self, x: torch.Tensor, xn: Optional[torch.Tensor] = None, _lib=None) -> torch.Tensor:
+    def forward(self, x: torch.Tensor, xn: Optional[torch.Tensor] = None, lengths=None, _lib=None) -> torch.Tensor:
+        """Gate the rows of x ([B, L]); xn: noise clip(s) for the stationary thresholds ([Ln], [1, Ln] or [B, Ln]).
+
+        lengths: a zero-padded batch of rows of different lengths (one int per row, a 1-D integer tensor or a sequence).
+        Row b is then gated as the signal x[b, :lengths[b]] alone: its first (lengths[b] // hop) * hop output samples
+        equal forward(x[b:b+1, :lengths[b]], xn_b)[0] in every bit (xn_b = xn, or its row b when xn has B rows), the
+        rest of the row is zero, samples of x past lengths[b] are never read, and the gradient past lengths[b] is zero.
+        The output keeps the shape of forward(x).  2 * win_length <= lengths[b] <= L.  A CUDA tensor of lengths is
+        read back to the host once, which waits for its stream; a CPU tensor or a list does not wait.  Covered: the
+        default STFT geometry (n_fft = win_length = 1024, hop 256), float32 / float16 / bfloat16 x, both gates; other
+        inputs raise NotImplementedError.  forward(x, lengths=[L] * B) is promised to equal forward(x) to float32
+        rounding only: the last bit at synthesis work-item seams may depend on how many rows share a call."""
         assert x.ndim == 2                                                      # torchgate.py:214-220
         if x.shape[-1] < self.win_length * 2:
             raise Exception(f"x must be bigger than {self.win_length * 2}")
@@ -108,15 +119,52 @@ class TorchGate(torch.nn.Module):
             raise Exception(f"xn must be bigger than {self.win_length * 2}")
         if _lib is None and not x.is_cuda:
             raise RuntimeError("noisereduce_b200.TorchGate runs on CUDA tensors only (no CPU fallback)")
+        if lengths is not None:
+            lengths = self._row_lengths(x, lengths)
         if torch.is_grad_enabled() and x.requires_grad:
             # torchgate.py:223-262: the masks are built under no_grad, the gradient flows through stft -> * mask -> istft
-            return _GateFunction.apply(x, self, xn, _lib)
-        return self._forward_impl(x, xn, _lib)[0]
+            return _GateFunction.apply(x, self, xn, lengths, _lib)
+        return self._forward_impl(x, xn, lengths, _lib)[0]
 
     def _tuned(self):
         return self.n_fft == 1024 and self.win_length == 1024 and self.hop_length == 256
 
-    def _forward_impl(self, x, xn, _lib):
+    def _row_lengths(self, x, lengths):
+        """The checked lengths= of forward() as a list of ints; raises before any library handle is made."""
+        if not self._tuned():
+            raise NotImplementedError("TorchGate.forward(lengths=...) needs the default STFT geometry (n_fft = win_length "
+                                      f"= 1024, hop_length = 256), not n_fft={self.n_fft}, win_length={self.win_length}, "
+                                      f"hop_length={self.hop_length}")
+        if x.dtype not in (torch.float32, torch.float16, torch.bfloat16):
+            raise NotImplementedError(f"TorchGate.forward(lengths=...) takes float32 / float16 / bfloat16 x, not {x.dtype}")
+        nf, nt = self._extents if self.smoothing_filter is not None else (0, 0)
+        reason = _rows_smoothing_refusal(nf, nt, self.nonstationary)
+        if reason:
+            raise NotImplementedError(f"TorchGate.forward(lengths=...): freq_mask_smooth_hz={self.freq_mask_smooth_hz} / "
+                                      f"time_mask_smooth_ms={self.time_mask_smooth_ms} give smoothing extents ({nf}, {nt}) "
+                                      f"bins / frames, {reason}")
+        if isinstance(lengths, torch.Tensor):
+            if lengths.ndim != 1 or lengths.dtype.is_floating_point or lengths.dtype.is_complex or lengths.dtype == torch.bool:
+                raise ValueError(f"lengths must be a 1-D integer tensor, got {tuple(lengths.shape)} {lengths.dtype}")
+            lengths = lengths.tolist()                          # (a CUDA tensor: one device -> host copy)
+        else:
+            try:
+                lengths = list(lengths)
+            except TypeError:
+                raise ValueError("lengths must be a 1-D integer tensor or a sequence of ints") from None
+            if not all(isinstance(n, (int, np.integer)) and not isinstance(n, (bool, np.bool_)) for n in lengths):
+                raise ValueError("lengths must be integers")
+            lengths = [int(n) for n in lengths]
+        B, L = x.shape
+        if len(lengths) != B:
+            raise ValueError(f"lengths has {len(lengths)} entries, x has {B} rows")
+        if max(lengths) > L:
+            raise ValueError(f"lengths ({max(lengths)}) beyond the {L} samples of x")
+        if min(lengths) < self.win_length * 2:
+            raise Exception(f"x must be bigger than {self.win_length * 2}")
+        return lengths
+
+    def _forward_impl(self, x, xn, lengths, _lib):
         f64 = x.dtype == torch.float64
         work_t, np_t = (torch.float64, np.float64) if f64 else (torch.float32, np.float32)
         ctx = torch.cuda.device(x.device) if x.is_cuda else _NullCtx()
@@ -132,8 +180,12 @@ class TorchGate(torch.nn.Module):
                 gate.torch_set_noise(None, 0, 0, 0, True, stream)
             B, L = xf.shape
             Lo = (L // self.hop_length) * self.hop_length + (self.n_fft & 1)     # torch.istft(center=True) length
-            y = torch.empty((B, Lo), dtype=work_t, device=x.device)
-            gate.run_device(xf.data_ptr(), y.data_ptr(), np_t, B, L, xf.stride(0), y.stride(0), stream)
+            if lengths is None:
+                y = torch.empty((B, Lo), dtype=work_t, device=x.device)
+                gate.run_device(xf.data_ptr(), y.data_ptr(), np_t, B, L, xf.stride(0), y.stride(0), stream)
+            else:                                               # b200gate_run_rows: row b is x[b, :lengths[b]] alone
+                y = torch.zeros((B, Lo), dtype=work_t, device=x.device)
+                gate.run_rows(_rows(xf, y, lengths), np_t, True, stream)
             gate._fwd_serial = getattr(gate, "_fwd_serial", 0) + 1
         return y.to(dtype=x.dtype), gate                                        # torchgate.py:264
 
@@ -146,6 +198,34 @@ class TorchGate(torch.nn.Module):
         idx = (torch.arange(T, device=device) * H)[:, None] + torch.arange(N, device=device)[None, :]
         env.index_add_(0, idx.reshape(-1), w2.repeat(T))
         return env[N // 2: N // 2 + (L // H) * H]
+
+    def _adjoint_rows(self, g, gate, serial, L, lengths, _lib):
+        """_adjoint of forward(x, lengths=...): row b is the map of its own lengths[b] samples, so its envelope is
+        _ola_envelope(lengths[b]) -- the single-row path's divisor -- and b200gate_torch_apply_masks_rows applies the
+        forward's masks row by row.  Input samples past a row's output length get a zero gradient."""
+        if getattr(gate, "_fwd_serial", 0) != serial:
+            raise RuntimeError("TorchGate.backward: another forward ran on this module since the forward being "
+                               "differentiated (its masks were overwritten); call backward first or use a second module")
+        B, Lo = g.shape
+        H = self.hop_length
+        env = torch.ones((B, Lo), dtype=torch.float32, device=g.device)
+        envs = {}
+        for b, n in enumerate(lengths):                         # one envelope per frame count
+            T = n // H
+            if T not in envs:
+                envs[T] = self._ola_envelope(n, g.device)
+            env[b, :T * H] = envs[T]
+        own = torch.arange(Lo, device=g.device)[None, :] < torch.tensor([(n // H) * H for n in lengths], device=g.device)[:, None]
+        z = torch.zeros((B, L), dtype=torch.float32, device=g.device)
+        z[:, :Lo] = torch.where(own, g.to(torch.float32) / env, 0.0)
+        out = torch.zeros((B, Lo), dtype=torch.float32, device=g.device)
+        ctx = torch.cuda.device(g.device) if g.is_cuda else _NullCtx()
+        with ctx:
+            stream = torch.cuda.current_stream(g.device).cuda_stream if g.is_cuda else None
+            gate.torch_apply_masks_rows(_rows(z, out, lengths), np.float32, True, stream)
+        grad = torch.zeros((B, L), dtype=torch.float32, device=g.device)
+        grad[:, :Lo] = out * env
+        return grad
 
     def _adjoint(self, g, gate, serial, L, _lib):
         """Gradient of forward with respect to x (masks fixed): the gate is  y = OLA(w B(w frame(x))) / env  with a
@@ -171,19 +251,42 @@ class TorchGate(torch.nn.Module):
 
 class _GateFunction(torch.autograd.Function):
     @staticmethod
-    def forward(ctx, x, module, xn, lib):
+    def forward(ctx, x, module, xn, lengths, lib):
         if not module._tuned() or x.dtype == torch.float64:
             raise NotImplementedError("noisereduce_b200.TorchGate: the backward pass exists for float32 / float16 input at the "
                                       "default STFT geometry (n_fft 1024, hop 256); use torch.no_grad() otherwise")
-        y, gate = module._forward_impl(x, xn, lib)
-        ctx.module, ctx.gate, ctx.lib = module, gate, lib
+        y, gate = module._forward_impl(x, xn, lengths, lib)
+        ctx.module, ctx.gate, ctx.lib, ctx.lengths = module, gate, lib, lengths
         ctx.serial, ctx.L, ctx.dtype = gate._fwd_serial, x.shape[-1], x.dtype
         return y
 
     @staticmethod
     def backward(ctx, g):
-        grad = ctx.module._adjoint(g.contiguous(), ctx.gate, ctx.serial, ctx.L, ctx.lib)
-        return grad.to(ctx.dtype), None, None, None
+        if ctx.lengths is None:
+            grad = ctx.module._adjoint(g.contiguous(), ctx.gate, ctx.serial, ctx.L, ctx.lib)
+        else:
+            grad = ctx.module._adjoint_rows(g.contiguous(), ctx.gate, ctx.serial, ctx.L, ctx.lengths, ctx.lib)
+        return grad.to(ctx.dtype), None, None, None, None
+
+
+def _rows(x, y, lengths):
+    """b200gate_row tuples (in, out, n, channels = 1) for float32 rows of x and y with unit sample stride."""
+    xs, ys = x.stride(0) * 4, y.stride(0) * 4
+    return [(x.data_ptr() + b * xs, y.data_ptr() + b * ys, int(n), 1) for b, n in enumerate(lengths)]
+
+
+def _rows_smoothing_refusal(nf, nt, nonstationary, f_pad=544, smem=200 * 1024):
+    """Why the rows form cannot smooth extents (nf, nt), or None.  (1) A filter whose integer numerators outgrow 16 bits
+    sends the library handle to the float64 general family, which has no rows form (big_filter in b200gate_create).
+    (2) The non-stationary gate's streaming smoothing keeps a ring of 2 nt + 1 mask rows in shared memory (k_smooth_box
+    for 1 <= nf <= 12, else k_smooth_stream; smoothb_smem_bytes / smooths_smem_bytes in gate_kernels.cuh)."""
+    if nf > 64 or nt > 64 or (nf + 1) ** 2 * (nt + 1) ** 2 > 65535:
+        return "beyond the 16-bit mask numerators of the n_fft 1024 kernels ((nf + 1)^2 (nt + 1)^2 <= 65535, at most 64 a side)"
+    box = ((2 * nt + 1) * f_pad + (f_pad + 32) + (f_pad + 16)) * 4
+    stream = ((2 * nt + 1) * f_pad + f_pad + 2 * nf + 8) * 4
+    if nonstationary and not ((1 <= nf <= 12 and box <= smem) or stream <= smem):
+        return "beyond the shared-memory ring of the non-stationary gate's smoothing"
+    return None
 
 
 class _NullCtx:
