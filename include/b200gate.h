@@ -148,6 +148,30 @@ int b200gate_channel_sum(b200gate_handle* h, const void* y, int dtype, int64_t C
                          void* cuda_stream);
 int b200gate_set_noise_threshold(b200gate_handle* h, const double* thresh_db, int32_t n_bins);
 int b200gate_get_noise_threshold(const b200gate_handle* h, double* thresh_db, int32_t n_bins);
+
+/* Per-recording stationary thresholds (reduce_noise_batch with a noise clip per item).
+ * b200gate_noise_stats_rows: the thresholds of n_clips noise clips, row r of thresh_out [n_clips][513] (host memory) in
+ * every bit what b200gate_noise_stats + b200gate_get_noise_threshold give for clip r on this handle.  Clip r is
+ * [C][n] samples of `dtype` with row stride `stride` elements, clipped to chunk_size when clip_noise is set, as
+ * b200gate_noise_stats does.  Device clips (is_device = 1) are read in place on cuda_stream; host clips may lie anywhere:
+ * their channel sums are taken on the host, in channel order as b200gate_noise_stats does, and only the sums are copied
+ * to the device, in one copy.  The clips run in groups whose float64 spectrograms fit the workspace limit
+ * (workspace_limit_bytes, or 70 % of the free device memory), one launch per kernel and group; the thresholds are read
+ * back once, and the call returns after that synchronise.  The handle's installed thresholds are not touched.
+ * B200GATE_ERR_ARG: a geometry other than n_fft = win_length = 1024, hop_length = 256 (or the general family), a clip
+ * with a null pointer, no channels or samples, a row stride below n for C > 1, or fewer than win_length samples after
+ * clipping (scipy shortens the window for such a clip: b200gate_noise_stats on a handle with win_length = n takes it). */
+typedef struct b200gate_noise_clip { const void* x; int64_t C; int64_t n; int64_t stride; } b200gate_noise_clip;
+int b200gate_noise_stats_rows(b200gate_handle* h, const b200gate_noise_clip* clips, int64_t n_clips, int dtype,
+                              int is_device, double* thresh_out, void* cuda_stream);
+/* b200gate_set_noise_threshold_rows: install one threshold row per recording, thresh_db [n_recordings][n_bins = 513],
+ * for the next b200gate_run_rows calls (see there).  The tables are built on the host with the arithmetic of
+ * b200gate_set_noise_threshold, so a recording's tables equal the ones its row would give as a single set, and go to the
+ * device in one copy.  While they are installed b200gate_run, a stationary stream, b200gate_get_noise_threshold and
+ * b200gate_get_noise_mean_std return B200GATE_ERR_STATE; b200gate_set_noise_threshold and b200gate_noise_stats return
+ * the handle to one set.  B200GATE_ERR_ARG: a handle other than a stationary numpy-surface gate at n_fft 1024, or
+ * n_bins != 513. */
+int b200gate_set_noise_threshold_rows(b200gate_handle* h, const double* thresh_db, int64_t n_recordings, int32_t n_bins);
 int b200gate_get_noise_mean_std(const b200gate_handle* h, double* mean_db, double* std_db, int32_t n_bins);
 
 /* Torch surfaces only: install the analysis/synthesis window the caller built with
@@ -180,7 +204,12 @@ int b200gate_run(b200gate_handle* h, const void* in, void* out, int dtype, int64
  * top_db row maxima, the non-stationary follower's sweeps and its choice between regenerating and storing the forward
  * sweep) are taken per row.  The channels of a multi-channel recording are simply consecutive rows: with the thresholds
  * fixed (b200gate_noise_stats / b200gate_set_noise_threshold, once for all rows) a channel's result depends on no other
- * channel in either gate.  The units of all rows share the workspace at the pitch of the call's longest unit.
+ * channel in either gate.  With per-recording thresholds installed (b200gate_set_noise_threshold_rows, stationary gate)
+ * the rows group into recordings in order: row 0 starts recording 0, and a recording is `channels` consecutive rows
+ * of equal n and channels; every unit of recording i compares against row i of the thresholds.  The number of
+ * recordings must equal the rows installed (B200GATE_ERR_ARG otherwise, as for a recording whose rows differ in n or
+ * channels or that runs past the last row).  With one set installed nothing of this applies.
+ * The units of all rows share the workspace at the pitch of the call's longest unit.
  * Device pointers (is_device = 1) are read and written where they are and the call only enqueues on cuda_stream, without
  * waiting for the device.  Host rows must lie in one buffer each way: they travel as the span that covers them, one copy
  * in and one copy out (bytes of the output span between rows are overwritten), and the call returns with the result in

@@ -38,7 +38,7 @@ EXPORTS = [
     "b200gate_host_alloc", "b200gate_host_free",
     "b200gate_stream_begin", "b200gate_stream_push", "b200gate_stream_finish", "b200gate_convert",
     "b200gate_mask_store_bytes", "b200gate_set_mask_store", "b200gate_adjoint", "b200gate_run_rows",
-    "b200gate_torch_apply_masks_rows",
+    "b200gate_torch_apply_masks_rows", "b200gate_noise_stats_rows", "b200gate_set_noise_threshold_rows",
 ]
 
 
@@ -73,6 +73,11 @@ class Stats(C.Structure):
 class Row(C.Structure):
     """b200gate_row: one channel of one recording (b200gate_run_rows)."""
     _fields_ = [("in_", C.c_void_p), ("out", C.c_void_p), ("n", C.c_int64), ("channels", C.c_int64)]
+
+
+class NoiseClip(C.Structure):
+    """b200gate_noise_clip: one noise clip of b200gate_noise_stats_rows, [C][n] with row stride `stride` elements."""
+    _fields_ = [("x", C.c_void_p), ("C", C.c_int64), ("n", C.c_int64), ("stride", C.c_int64)]
 
 
 class GateError(RuntimeError):
@@ -139,6 +144,8 @@ class GateLibrary:
         d.b200gate_adjoint.argtypes = [vp, vp, vp, vp, C.c_int, i64, i64, i64, i64, C.c_int, vp]
         d.b200gate_run_rows.argtypes = [vp, C.POINTER(Row), i64, C.c_int, C.c_int, vp]
         d.b200gate_torch_apply_masks_rows.argtypes = [vp, C.POINTER(Row), i64, C.c_int, C.c_int, vp]
+        d.b200gate_noise_stats_rows.argtypes = [vp, C.POINTER(NoiseClip), i64, C.c_int, C.c_int, C.POINTER(dbl), vp]
+        d.b200gate_set_noise_threshold_rows.argtypes = [vp, C.POINTER(dbl), i64, i32]
 
 
 def format_code(dt) -> int:
@@ -301,6 +308,20 @@ class Gate:
         t = np.ascontiguousarray(thresh_db, dtype=np.float64)
         self._check(self.lib.dll.b200gate_set_noise_threshold(
             self._h, t.ctypes.data_as(C.POINTER(C.c_double)), t.shape[0]))
+
+    def noise_stats_rows(self, clips, dtype, is_device, stream=None) -> np.ndarray:
+        """b200gate_noise_stats_rows on (ptr, C, n, stride) tuples of one dtype; returns the thresholds [len(clips)][n_bins]."""
+        arr = (NoiseClip * len(clips))(*clips)
+        out = np.empty((len(clips), self.n_bins), dtype=np.float64)
+        self._check(self.lib.dll.b200gate_noise_stats_rows(self._h, arr, len(clips), dtype_code(dtype), 1 if is_device else 0,
+                                                           out.ctypes.data_as(C.POINTER(C.c_double)), stream))
+        return out
+
+    def set_noise_threshold_rows(self, thresh_db):
+        """b200gate_set_noise_threshold_rows: one threshold row per recording of the next run_rows calls."""
+        t = np.ascontiguousarray(thresh_db, dtype=np.float64)
+        self._check(self.lib.dll.b200gate_set_noise_threshold_rows(
+            self._h, t.ctypes.data_as(C.POINTER(C.c_double)), t.shape[0], t.shape[1]))
 
     def noise_threshold(self) -> np.ndarray:
         out = np.empty(self.n_bins, dtype=np.float64)

@@ -62,6 +62,11 @@ struct b200gate_handle {
     int tthr_units = 0;
     bool have_thresh = false;
     double min_floor_amp = 0.0;                    // min_f 10^((thresh+top_db)/20): smallest |X| that lifts a row
+    // b200gate_set_noise_threshold_rows: n_rec > 0 recordings' tables in one device buffer (have_thresh is then false):
+    // thr4 | gco | floor4 as [n_rec][FPad] float, then thr2_64 as [n_rec][F] double (rec_tables())
+    int n_rec = 0;
+    void* d_rtab = nullptr;
+    size_t rtab_bytes = 0;
     int range_mode = 0;                            // b200gate_set_range
     long long range_a = 0, range_b = 0;
     std::vector<double> thr, mean, sd;
@@ -342,27 +347,47 @@ int build_static_tables(b200gate_handle* h) {
 
 // Tables that depend on the noise threshold (stationary.py:79-81), in the linear power domain:
 // dB > thresh  <=>  |X| + eps > 10^(thresh/20)  <=>  |X|^2 > T_amp^2.
+// One recording's rows from its thresholds thr[F] into thr4 / gco / floor4 [FPad] (pads left as they are) and t2 [F];
+// returns min_floor_amp.  The single set and the per-recording tables both come from here, so they hold the same bits.
+double threshold_rows(const b200gate_params& p, const double* thr, float* thr4, float* gco, float* floor4, double* t2) {
+    double min_floor_amp = 0.0;
+    for (int f = 0; f < kF; ++f) {
+        double T = pow(10.0, thr[f] / 20.0) - kEps64;
+        if (!(T > 0.0)) T = 0.0;
+        double Tf = pow(10.0, (thr[f] + p.top_db) / 20.0) - kEps64;
+        if (!(Tf > 0.0)) Tf = 0.0;
+        t2[f] = T * T;
+        if (f == 0 || Tf < min_floor_amp) min_floor_amp = Tf;
+        thr4[f] = (float)(4.0 * T * T);
+        gco[f] = (float)(8.0 * T * kKappa * kEps32 * (p.debug_guard_scale > 0 ? p.debug_guard_scale : 1));
+        floor4[f] = (float)(4.0 * Tf * Tf);
+    }
+    return min_floor_amp;
+}
+
 int build_threshold_tables(b200gate_handle* h) {
     std::vector<float> thr4(kFPad, INFINITY), gco(kFPad, 0.f), floor4(kFPad, INFINITY);
     std::vector<double> t2(kF);
-    for (int f = 0; f < kF; ++f) {
-        double T = pow(10.0, h->thr[f] / 20.0) - kEps64;
-        if (!(T > 0.0)) T = 0.0;
-        double Tf = pow(10.0, (h->thr[f] + h->p.top_db) / 20.0) - kEps64;
-        if (!(Tf > 0.0)) Tf = 0.0;
-        t2[f] = T * T;
-        if (f == 0 || Tf < h->min_floor_amp) h->min_floor_amp = Tf;
-        thr4[f] = (float)(4.0 * T * T);
-        gco[f] = (float)(8.0 * T * kKappa * kEps32 * (h->p.debug_guard_scale > 0 ? h->p.debug_guard_scale : 1));
-        floor4[f] = (float)(4.0 * Tf * Tf);
-    }
+    h->min_floor_amp = threshold_rows(h->p, h->thr.data(), thr4.data(), gco.data(), floor4.data(), t2.data());
     int rc;
     if ((rc = upload(h, &h->d_thr4, thr4))) return rc;
     if ((rc = upload(h, &h->d_gco, gco))) return rc;
     if ((rc = upload(h, &h->d_floor4, floor4))) return rc;
     if ((rc = upload(h, &h->d_thr2_64, t2))) return rc;
     h->have_thresh = true;
+    h->n_rec = 0;                                  // (a single set replaces per-recording thresholds)
     return B200GATE_OK;
+}
+
+// the device tables of per-recording thresholds (b200gate_set_noise_threshold_rows) in the layout of h->d_rtab
+Tables rec_tables(const b200gate_handle* h, Tables tb) {
+    const size_t R = (size_t)h->n_rec;
+    float* f = (float*)h->d_rtab;
+    tb.thr4 = f;
+    tb.gco = f + R * kFPad;
+    tb.floor4 = f + 2 * R * kFPad;
+    tb.thr2_64 = (const double*)(f + 3 * R * kFPad);
+    return tb;
 }
 
 Tables device_tables(const b200gate_handle* h) {
@@ -1009,6 +1034,8 @@ int b200gate_create(const b200gate_params* p, b200gate_handle** out) {
             B200_WITH_DTYPE(dt, {
                 cudaFuncSetAttribute(k1_analyze<8, T, false, true>, cudaFuncAttributeMaxDynamicSharedMemorySize, k1_smem_floats() * 4);
                 cudaFuncSetAttribute(k1_analyze<8, T, true, true>, cudaFuncAttributeMaxDynamicSharedMemorySize, k1_smem_floats() * 4);
+                cudaFuncSetAttribute(k1_analyze<8, T, false, true, true>, cudaFuncAttributeMaxDynamicSharedMemorySize, k1_smem_floats() * 4);
+                cudaFuncSetAttribute(k1_analyze<8, T, true, true, true>, cudaFuncAttributeMaxDynamicSharedMemorySize, k1_smem_floats() * 4);
                 cudaFuncSetAttribute(k1n_magnitude<8, T, true>, cudaFuncAttributeMaxDynamicSharedMemorySize, k1n_smem_floats() * 4);
                 cudaFuncSetAttribute(k2c_synthesize<8, kMaskF32, T, true>, cudaFuncAttributeMaxDynamicSharedMemorySize, k2c_smem_bytes<kMaskF32>());
                 cudaFuncSetAttribute(k2c_synthesize<8, kMaskBits, T, true>, cudaFuncAttributeMaxDynamicSharedMemorySize, k2c_smem_bytes<kMaskBits>());
@@ -1072,6 +1099,7 @@ void b200gate_destroy(b200gate_handle* h) {
     if (h->d_need_rowmax) cudaFree(h->d_need_rowmax);
     g_pinned_pool.give(h->hp_units, h->hp_units_bytes);
     if (h->d_units) cudaFree(h->d_units);
+    if (h->d_rtab) cudaFree(h->d_rtab);
     if (h->ev_units) cudaEventDestroy(h->ev_units);
     for (cudaEvent_t e : h->stage_ev) cudaEventDestroy(e);
     for (cudaEvent_t e : h->pipe_ev) cudaEventDestroy(e);
@@ -1100,6 +1128,42 @@ int b200gate_set_noise_threshold(b200gate_handle* h, const double* thresh_db, in
         return rc;
     }
     return build_threshold_tables(h);
+}
+
+int b200gate_set_noise_threshold_rows(b200gate_handle* h, const double* thresh_db, int64_t n_recordings, int32_t n_bins) {
+    if (!h || !thresh_db || n_recordings <= 0) return fail(h, B200GATE_ERR_ARG, "bad argument");
+    const b200gate_params& p = h->p;
+    if (!p.stationary || p.surface != B200GATE_SURFACE_NUMPY || h->generic || p.n_fft != kN)
+        return fail(h, B200GATE_ERR_ARG, "per-recording thresholds are for the stationary numpy-surface gate at n_fft 1024");
+    if (n_bins != kF) return fail(h, B200GATE_ERR_ARG, "expected %d bins, got %d", kF, n_bins);
+    if (n_recordings > 0x7fffffffLL / kFPad) return fail(h, B200GATE_ERR_ARG, "too many recordings");
+    const size_t R = (size_t)n_recordings;
+    // one host image of the tables (the layout of rec_tables()), one upload
+    const size_t fl = 3 * R * kFPad;                       // (3 kFPad floats are a whole number of doubles)
+    std::vector<double> img(fl / 2 + R * kF);
+    float* f = (float*)img.data();
+    double* t2 = img.data() + fl / 2;
+    for (size_t r = 0; r < R; ++r) {
+        float *thr4 = f + r * kFPad, *gco = f + (R + r) * kFPad, *floor4 = f + (2 * R + r) * kFPad;
+        std::fill(thr4, thr4 + kFPad, INFINITY);
+        std::fill(gco, gco + kFPad, 0.f);
+        std::fill(floor4, floor4 + kFPad, INFINITY);
+        const double mfa = threshold_rows(p, thresh_db + r * kF, thr4, gco, floor4, t2 + r * kF);
+        floor4[kFPad - 1] = (float)(4.0 * mfa * mfa);      // the recording's need_rowmax guard (k1_analyze<.., PERREC>)
+    }
+    const size_t bytes = img.size() * sizeof(double);
+    if (h->rtab_bytes < bytes) {
+        if (h->d_rtab) cudaFree(h->d_rtab);
+        h->d_rtab = nullptr;
+        h->rtab_bytes = 0;
+        h->n_rec = 0;
+        CK(h, cudaMalloc(&h->d_rtab, bytes));
+        h->rtab_bytes = bytes;
+    }
+    CK(h, cudaMemcpy(h->d_rtab, img.data(), bytes, cudaMemcpyHostToDevice));
+    h->n_rec = (int)R;
+    h->have_thresh = false;                                // (b200gate_run, get_noise_threshold, streams: ERR_STATE)
+    return B200GATE_OK;
 }
 
 int b200gate_get_noise_threshold(const b200gate_handle* h, double* thresh_db, int32_t n_bins) {
@@ -1254,6 +1318,156 @@ int b200gate_noise_stats(b200gate_handle* h, const void* y_noise, int dtype, int
         rc = noise_stats_from_mean(h, d_yn, n, st);
     }
     return rc;
+}
+
+}  // extern "C"
+
+namespace {
+// host clips: channel-order sums of samples [i0, i1) into a, the additions of channel_sum_impl's host path
+template <typename Tin, typename Tacc>
+void host_channel_sum(const Tin* y, long long C, long long stride, long long i0, long long i1, Tacc* a) {
+    for (long long i = i0; i < i1; ++i) a[i] = (Tacc)0;
+    for (long long c = 0; c < C; ++c) {
+        const Tin* r = y + c * stride;
+        for (long long i = i0; i < i1; ++i) a[i] = a[i] + (Tacc)r[i];
+    }
+}
+}  // namespace
+
+extern "C" {
+
+// Thresholds of many clips: one K0Clip table, then per group of clips (under the workspace limit) one launch each of
+// k0_clip_mean_rows, k0_stft_db_rows and k0_stats_rows; the thresholds of every clip are read back at the end, once.
+int b200gate_noise_stats_rows(b200gate_handle* h, const b200gate_noise_clip* clips, int64_t n_clips, int dtype,
+                              int is_device, double* thresh_out, void* stream) {
+    if (!h || !clips || n_clips <= 0 || !thresh_out || dtype_size(dtype) == 0) return fail(h, B200GATE_ERR_ARG, "bad argument");
+    const b200gate_params& p = h->p;
+    if (h->generic || p.n_fft != kN || p.win_length != kN || p.hop_length != kN / 4)
+        return fail(h, B200GATE_ERR_ARG, "b200gate_noise_stats_rows needs n_fft = win_length = 1024, hop_length = 256");
+    cudaStream_t st = (cudaStream_t)stream;
+    const int H = p.hop_length;
+    const bool f32 = dtype == B200GATE_F32;
+    const size_t as = f32 ? 4 : 8;                             // accumulation dtype of the channel sum
+    std::vector<K0Clip> tab((size_t)n_clips);
+    long long n_sum = 0;                                       // host clips: samples of all their channel sums
+    for (int64_t r = 0; r < n_clips; ++r) {
+        const b200gate_noise_clip& c = clips[r];
+        if (!c.x || c.C <= 0 || c.n <= 0 || (c.C > 1 && c.stride < c.n))
+            return fail(h, B200GATE_ERR_ARG, "clip %lld: null pointer, no samples or channels, or a row stride below n", (long long)r);
+        long long n = c.n;
+        if (p.clip_noise && p.chunk_size > 0 && n > p.chunk_size) n = p.chunk_size;       // stationary.py:63-64
+        if (n < p.win_length)                                  // (scipy would shorten the window: b200gate_noise_stats on
+            return fail(h, B200GATE_ERR_ARG, "clip %lld: %lld samples after clipping, fewer than win_length %d "
+                        "(b200gate_noise_stats takes such a clip on a handle with win_length = n)", (long long)r, n, p.win_length);
+        K0Clip& k = tab[(size_t)r];
+        k.x = c.x; k.stride = c.stride; k.c_sum = c.C; k.C = c.C; k.n = n; k.Tn = (int)(n / H) + 1;
+        if (!is_device) {                                      // (x is set to the device copy of its sums below)
+            k.yn_off = n_sum;
+            n_sum += n;
+        }
+    }
+    // host clips: their channel sums are taken by the host workers, the same additions in the same type as
+    // k0_channel_sum, and only the sums travel, with the table, in one pinned buffer and one copy
+    const size_t tab_bytes = tab.size() * sizeof(K0Clip), sum_off = (tab_bytes + 255) / 256 * 256;
+    const size_t up_bytes = sum_off + (is_device ? 0 : (size_t)n_sum * as);
+    size_t pinned_bytes = 0;
+    void* hp = g_pinned_pool.take(up_bytes, &pinned_bytes);
+    if (!hp) return fail(h, B200GATE_ERR_NOMEM, "pinned staging (%zu bytes)", up_bytes);
+    struct PinnedBack {
+        void* p; size_t b;
+        ~PinnedBack() { g_pinned_pool.give(p, b); }            // (after the synchronise below, or on an early return)
+    } pinned_back{hp, pinned_bytes};
+    Scratch s_up;
+    CK(h, s_up.alloc(up_bytes));
+    const K0Clip* d_tab = s_up.as<K0Clip>();
+    if (!is_device) {
+        unsigned char* hsum = (unsigned char*)hp + sum_off;
+        const long long blk = 8192;
+        std::vector<std::pair<int64_t, long long>> jobs;        // (clip, first sample of a block)
+        for (int64_t r = 0; r < n_clips; ++r)
+            for (long long i0 = 0; i0 < tab[(size_t)r].n; i0 += blk) jobs.emplace_back(r, i0);
+        const int nt = (int)std::max<size_t>(1, std::min<size_t>((size_t)std::min(h->host_threads, 32), jobs.size()));
+        std::function<void(int)> work = [&](int id) {
+            for (size_t j = (size_t)id; j < jobs.size(); j += (size_t)nt) {
+                const K0Clip& k = tab[(size_t)jobs[j].first];
+                const long long i0 = jobs[j].second, i1 = std::min(k.n, i0 + blk);
+                void* a = hsum + (size_t)k.yn_off * as;
+                if (dtype == B200GATE_F32) host_channel_sum((const float*)k.x, k.C, k.stride, i0, i1, (float*)a);
+                else if (dtype == B200GATE_I16) host_channel_sum((const short*)k.x, k.C, k.stride, i0, i1, (double*)a);
+                else host_channel_sum((const double*)k.x, k.C, k.stride, i0, i1, (double*)a);
+            }
+        };
+        host_workers(0).run(nt, work);
+        for (K0Clip& k : tab) {
+            k.x = (const char*)s_up.p + sum_off + (size_t)k.yn_off * as;
+            k.stride = k.n;
+            k.c_sum = 1;
+        }
+    }
+    // groups of clips whose float64 means and dB spectrograms fit the workspace limit (at least one clip each)
+    double limit = p.workspace_limit_bytes;
+    if (!(limit > 0)) {
+        limit = 24.0 * 1024 * 1024 * 1024;
+        size_t free_b = 0, total_b = 0;
+        if (cudaMemGetInfo(&free_b, &total_b) == cudaSuccess) limit = std::min(limit, 0.7 * (double)free_b);
+    }
+    std::vector<int64_t> g_start{0};
+    long long yn_max = 0, t_max = 0;
+    {
+        long long yn = 0, t = 0;
+        for (int64_t r = 0; r < n_clips; ++r) {
+            K0Clip& k = tab[(size_t)r];
+            const double more = 8.0 * ((double)(yn + k.n) + (double)(t + k.Tn) * kF);
+            if (r > g_start.back() && (more > limit || r - g_start.back() >= 65535 || t + k.Tn > 0x7fffffffLL)) {
+                g_start.push_back(r);
+                yn = t = 0;
+            }
+            k.yn_off = yn;                                     // (host clips' sums were placed above: x holds them)
+            k.t_off = t;
+            yn += k.n;
+            t += k.Tn;
+            yn_max = std::max(yn_max, yn);
+            t_max = std::max(t_max, t);
+        }
+        g_start.push_back(n_clips);
+    }
+    Scratch s_yn, s_db, s_res;
+    CK(h, s_yn.alloc((size_t)yn_max * sizeof(double)));
+    CK(h, s_db.alloc((size_t)t_max * kF * sizeof(double)));
+    CK(h, s_res.alloc((size_t)n_clips * 3 * kF * sizeof(double)));
+    memcpy(hp, tab.data(), tab_bytes);
+    CK(h, cudaMemcpyAsync(s_up.p, hp, up_bytes, cudaMemcpyHostToDevice, st));
+    double *d_yn = s_yn.as<double>(), *d_db = s_db.as<double>(), *d_res = s_res.as<double>();
+    for (size_t gi = 0; gi + 1 < g_start.size(); ++gi) {
+        const int64_t c0 = g_start[gi], nc = g_start[gi + 1] - c0;
+        long long n_hi = 0, frames = 0;
+        for (int64_t r = c0; r < c0 + nc; ++r) {
+            n_hi = std::max(n_hi, tab[(size_t)r].n);
+            frames += tab[(size_t)r].Tn;
+        }
+        const dim3 gm(grid_1d(n_hi, 256, std::max(1, 4096 / (int)nc)), (unsigned)nc);
+        if (f32) {
+            auto kern_ = k0_clip_mean_rows<float, float>;
+            B200_LAUNCH(kern_, gm, dim3(256), 0, st, d_tab + c0, d_yn);
+        } else if (dtype == B200GATE_I16 && is_device) {
+            auto kern_ = k0_clip_mean_rows<short, double>;
+            B200_LAUNCH(kern_, gm, dim3(256), 0, st, d_tab + c0, d_yn);
+        } else {
+            auto kern_ = k0_clip_mean_rows<double, double>;
+            B200_LAUNCH(kern_, gm, dim3(256), 0, st, d_tab + c0, d_yn);
+        }
+        K0Args a{};
+        a.yn = d_yn; a.H = H; a.wa64 = h->d_wa64; a.cs64 = h->d_cs64; a.eps = kEps64; a.db = d_db;
+        B200_LAUNCH(k0_stft_db_rows, dim3((unsigned)frames), dim3(256), kN * sizeof(double2), st, a, d_tab + c0, (int)nc);
+        B200_LAUNCH(k0_stats_rows, dim3(kF, (unsigned)nc), dim3(256), 0, st, d_db, d_tab + c0, p.top_db, p.std_ddof,
+                    p.n_std_thresh, d_res + (size_t)c0 * 3 * kF);
+        CK(h, cudaGetLastError());
+    }
+    // the thresholds: row 2 of every clip's [3][F] result
+    CK(h, cudaMemcpy2DAsync(thresh_out, kF * sizeof(double), d_res + 2 * kF, 3 * kF * sizeof(double), kF * sizeof(double),
+                            (size_t)n_clips, cudaMemcpyDeviceToHost, st));
+    CK(h, cudaStreamSynchronize(st));
+    return B200GATE_OK;
 }
 
 int b200gate_debug_select_unit(b200gate_handle* h, int64_t chunk, int64_t channel) {
@@ -1481,6 +1695,9 @@ static int run_core(b200gate_handle* h, const void* in, void* out, int dtype, in
     if (torch_rows && N < 2 * h->p.win_length) return fail(h, B200GATE_ERR_ARG, "x must be bigger than %d", 2 * h->p.win_length);
     if (torch_sem && h->tthr_units > 1 && h->tthr_units != C)
         return fail(h, B200GATE_ERR_ARG, "xn has %d rows, x has %lld", h->tthr_units, (long long)C);
+    if (h->p.stationary && !torch_sem && h->n_rec > 0)
+        return fail(h, B200GATE_ERR_STATE, "per-recording thresholds are installed; they serve b200gate_run_rows only "
+                    "(b200gate_set_noise_threshold or b200gate_noise_stats returns to one set)");
     if (h->p.stationary && !torch_sem && !h->have_thresh)
         return fail(h, B200GATE_ERR_STATE, "stationary gate: call b200gate_noise_stats first");
     cudaStream_t st = (cudaStream_t)stream;
@@ -2403,7 +2620,10 @@ int b200gate_run_rows(b200gate_handle* h, const b200gate_row* rows, int64_t n_ro
         return fail(h, B200GATE_ERR_ARG, "b200gate_run_rows: stationary smoothing extents (%d, %d) beyond the in-synthesis smoothing", nf, nt);
     if (!stat && !((nf >= 1 && nf <= 12 && smoothb_smem_bytes(kFPad, nt) <= 200 * 1024) || smooths_smem_bytes(kFPad, nf, nt) <= 200 * 1024))
         return fail(h, B200GATE_ERR_ARG, "b200gate_run_rows: smoothing extents (%d, %d) beyond the streaming smoothing kernels", nf, nt);
-    if (stat && !torch && !h->have_thresh) return fail(h, B200GATE_ERR_STATE, "stationary gate: call b200gate_noise_stats first");
+    // per-recording thresholds (b200gate_set_noise_threshold_rows): every unit reads its recording's rows of the tables
+    const bool perrec = stat && !torch && h->n_rec > 0;
+    if (stat && !torch && !h->have_thresh && !perrec)
+        return fail(h, B200GATE_ERR_STATE, "stationary gate: call b200gate_noise_stats first");
     if (torch && h->tthr_units > 1 && h->tthr_units != n_rows)
         return fail(h, B200GATE_ERR_ARG, "xn has %d rows, the call has %lld", h->tthr_units, (long long)n_rows);
     cudaStream_t st = (cudaStream_t)stream;
@@ -2437,6 +2657,21 @@ int b200gate_run_rows(b200gate_handle* h, const b200gate_row* rows, int64_t n_ro
         row_bytes += nb;
     }
     if (U > 0x7fffffffLL) return fail(h, B200GATE_ERR_ARG, "problem too large");
+    if (perrec) {                  // rows group into recordings in order: `channels` consecutive rows of equal n and channels
+        long long groups = 0;
+        for (int64_t r = 0; r < n_rows; r += rows[r].channels, ++groups) {
+            const int64_t k = rows[r].channels;
+            if (k > n_rows - r)
+                return fail(h, B200GATE_ERR_ARG, "row %lld starts a recording of %lld channels, %lld rows follow",
+                            (long long)r, (long long)k, (long long)(n_rows - r));
+            for (int64_t j = r + 1; j < r + k; ++j)
+                if (rows[j].n != rows[r].n || rows[j].channels != k)
+                    return fail(h, B200GATE_ERR_ARG, "row %lld: the channels of the recording from row %lld differ in n "
+                                "or channels", (long long)j, (long long)r);
+        }
+        if (groups != h->n_rec)
+            return fail(h, B200GATE_ERR_ARG, "the rows form %lld recordings, %d have thresholds", groups, h->n_rec);
+    }
     // host rows travel as the two spans that cover them, one copy each way: they must come packed in one buffer
     const size_t in_span = (size_t)(in_hi - in_lo), out_span = (size_t)(out_hi - out_lo);
     if (!is_device && std::max(in_span, out_span) > 2 * row_bytes + 4096 * (size_t)n_rows)
@@ -2472,8 +2707,10 @@ int b200gate_run_rows(b200gate_handle* h, const b200gate_row* rows, int64_t n_ro
     std::vector<long long> zero_units;                          // units whose centre reaches past their istft output
     {
         long long u = 0;
-        for (int64_t r = 0; r < n_rows; ++r) {
+        int rec = -1;                                           // perrec: the row's recording
+        for (int64_t r = 0, left = 0; r < n_rows; ++r, --left) {
             const b200gate_row& rw = rows[r];
+            if (left == 0) { ++rec; left = rw.channels; }
             const bool chunked = cs > 0 && rw.n > cs;
             const long long step = chunked ? cs : rw.n, nch = chunked ? (rw.n - 1) / cs + 1 : 1;
             const void* x = is_device ? rw.in : (const void*)((const char*)h->d_in + ((const char*)rw.in - in_lo));
@@ -2495,6 +2732,7 @@ int b200gate_run_rows(b200gate_handle* h, const b200gate_row* rows, int64_t n_ro
                     d.tf_hi = std::min(h_hi, d.T);
                 }
                 d.regen = stat || torch ? 0 : iir_regen_ok(b_iir, d.T, 0);
+                if (perrec) d.rec = rec;
                 // stationary.py:126 leaves the tail zero (a torch row's output ends with its istft length)
                 if (!torch && pad + step > sig_len) zero_units.push_back(u);
                 {   // hops per synthesis work item: run_core's choice for a [channels][n] recording in one workspace batch
@@ -2679,14 +2917,27 @@ int b200gate_run_rows(b200gate_handle* h, const b200gate_row* rows, int64_t n_ro
             a1.need_rowmax = h->d_need_rowmax;
             a1.min_floor4 = (float)(4.0 * h->min_floor_amp * h->min_floor_amp);
             const unsigned grid1 = (unsigned)grid_1d((long long)nu * n_runs1, kWarps, h->num_sm * B200_K1_MINBLOCKS);
-            B200_WITH_DTYPE(dtype, { auto kern_ = k1_analyze<8, T, false, true>;
-                B200_LAUNCH(kern_, dim3(grid1), dim3(kThreads), k1_smem_floats() * 4, st, a1); });
-            a1.guard = h->d_need_rowmax;                        // the row-maximum fallback, as in run_core
-            a1.zcache = nullptr;
-            B200_WITH_DTYPE(dtype, { auto kern_ = k1_analyze<8, T, true, true>;
-                B200_LAUNCH(kern_, dim3(grid1), dim3(kThreads), k1_smem_floats() * 4, st, a1); });
-            B200_LAUNCH(k_rowfloor, dim3(grid_1d((long long)nu * kFW, 256, 1 << 30)), dim3(256), 0, st, nu,
-                        (const unsigned*)d_rowmax, (const float*)h->d_floor4, d_rowflag, h->d_cnt);
+            const dim3 grid_rf(grid_1d((long long)nu * kFW, 256, 1 << 30));
+            if (perrec) {                                       // each unit reads its recording's rows of the tables
+                a1.tb = rec_tables(h, tb);
+                B200_WITH_DTYPE(dtype, { auto kern_ = k1_analyze<8, T, false, true, true>;
+                    B200_LAUNCH(kern_, dim3(grid1), dim3(kThreads), k1_smem_floats() * 4, st, a1); });
+                a1.guard = h->d_need_rowmax;
+                a1.zcache = nullptr;
+                B200_WITH_DTYPE(dtype, { auto kern_ = k1_analyze<8, T, true, true, true>;
+                    B200_LAUNCH(kern_, dim3(grid1), dim3(kThreads), k1_smem_floats() * 4, st, a1); });
+                B200_LAUNCH(k_rowfloor_rec, grid_rf, dim3(256), 0, st, nu, d_units + u0, (const unsigned*)d_rowmax,
+                            a1.tb.floor4, d_rowflag, h->d_cnt);
+            } else {
+                B200_WITH_DTYPE(dtype, { auto kern_ = k1_analyze<8, T, false, true>;
+                    B200_LAUNCH(kern_, dim3(grid1), dim3(kThreads), k1_smem_floats() * 4, st, a1); });
+                a1.guard = h->d_need_rowmax;                    // the row-maximum fallback, as in run_core
+                a1.zcache = nullptr;
+                B200_WITH_DTYPE(dtype, { auto kern_ = k1_analyze<8, T, true, true>;
+                    B200_LAUNCH(kern_, dim3(grid1), dim3(kThreads), k1_smem_floats() * 4, st, a1); });
+                B200_LAUNCH(k_rowfloor, grid_rf, dim3(256), 0, st, nu,
+                            (const unsigned*)d_rowmax, (const float*)h->d_floor4, d_rowflag, h->d_cnt);
+            }
             launches += 3;
             cudaEventRecord(h->stage_ev[4 * bi + 1], st);
             cudaEventRecord(h->stage_ev[4 * bi + 2], st);

@@ -62,7 +62,11 @@ struct UnitDesc {
     long long o_lo, o_hi;   // samples of the row this unit writes
     int T;                  // frames: Lp / H + 1
     int tf_hi;              // masks are needed for frames [tf_lo, tf_hi) (tf_lo is the same for every unit)
-    int regen;              // k_iir_sigmoid: iir_regen_ok of this unit's T
+    union {
+        int regen;          // non-stationary gate, k_iir_sigmoid: iir_regen_ok of this unit's T
+        int rec;            // stationary gate with per-recording thresholds (k1_analyze<.., PERREC>, k_rowfloor_rec):
+                            // the unit's recording, its row of the threshold tables
+    };
     int run;                // k2c_synthesize: output hops per work item, as run_core sizes them for this unit's recording
 };
 
@@ -76,6 +80,8 @@ struct Tables {              // device pointers, built once per handle
     const float* floor4;     // [FPad] 4 * (10^((thresh + top_db)/20) - eps)^2
     const float* ef;         // [FPad] frequency edge factor of the smoothing filter
     const double* thr2_64;   // [F]  T_amp^2 in float64
+    // (per-recording thresholds, b200gate_set_noise_threshold_rows: thr4 / gco / floor4 are [R][FPad] and thr2_64 is
+    //  [R][F], one row per recording; slot FPad - 1 of a floor4 row holds the recording's min_floor4, see K1Args)
     const double* wa64;      // [N]  analysis window / sum(w), float64
     const double2* cs64;     // [N]  (cos, sin)(2 pi m / N), float64
     float ws_to_w;           // raw window = ws * ws_to_w
@@ -378,7 +384,8 @@ struct K1Args {
     const unsigned* guard;     // optional device flag: when given and zero the kernel returns at once (it is then the
                                // row-maximum fallback behind k1_analyze<.., false> or k1d_analyze, gate_dual.cuh)
     unsigned* need_rowmax;     // k1_analyze<.., false>: device flag raised when a frame could reach its top_db floor
-    float min_floor4;          // min over bins of 4 * (10^((thresh + top_db)/20) - eps)^2
+    float min_floor4;          // min over bins of 4 * (10^((thresh + top_db)/20) - eps)^2 (PERREC: per recording, in
+                               // slot FPad - 1 of its floor4 row)
     const UnitDesc* units;     // ROWS instantiations: the call's unit table
 };
 
@@ -393,9 +400,13 @@ constexpr int k1_smem_floats() {
 // raises need_rowmax when a pair's energy could reach the lowest floor (|X_k|^2 <= N ||frame||^2), and the host then runs
 // the ROWMAX = true instantiation behind it (guarded by that flag) for the maxima.  That instantiation loads the samples
 // directly and tracks the maxima of every bin; run alone it is the whole analysis.
-template <int HR, typename T, bool ROWMAX = false, bool ROWS = false>
+// PERREC (with ROWS; b200gate_set_noise_threshold_rows): every unit compares against its recording's row of the
+// threshold tables (UnitDesc::rec), read through the read-only data path instead of the block's shared copy -- a
+// block's warps work on units of different recordings, and four per-warp copies would not fit next to the FFT tiles.
+template <int HR, typename T, bool ROWMAX = false, bool ROWS = false, bool PERREC = false>
 __global__ void __launch_bounds__(kThreads, B200_K1_MINBLOCKS) k1_analyze(const K1Args a) {
     static_assert(32 * (32 + HR) * 4 + 16 <= kK1WinBytes, "sample window must fit the buffer");
+    static_assert(ROWS || !PERREC, "per-recording thresholds need the unit table");
     constexpr bool kBulk = !ROWMAX && sizeof(T) <= 4;   // float32 / int16 windows (float64: direct loads)
     if (a.guard && *a.guard == 0u) return;
     B200_DYN_SMEM(float, smem);
@@ -411,9 +422,11 @@ __global__ void __launch_bounds__(kThreads, B200_K1_MINBLOCKS) k1_analyze(const 
         s_wa[i] = a.tb.wa[i];
         s_tw[i] = a.tb.tw[i];
     }
-    for (int i = threadIdx.x; i < kFPad; i += kThreads) {
-        s_thr4[i] = a.tb.thr4[i];
-        s_gco[i] = a.tb.gco[i];
+    if (!PERREC) {
+        for (int i = threadIdx.x; i < kFPad; i += kThreads) {
+            s_thr4[i] = a.tb.thr4[i];
+            s_gco[i] = a.tb.gco[i];
+        }
     }
     const Geom& g = a.g;
     const int lane = threadIdx.x & 31, warp = threadIdx.x >> 5;
@@ -492,6 +505,7 @@ __global__ void __launch_bounds__(kThreads, B200_K1_MINBLOCKS) k1_analyze(const 
         long long i1;
         unit_row(ul, xrow, i1);
         const long long Lp_u = unit_Lp(ul), n_u = unit_n(ul);
+        const int rec = PERREC ? a.units[g.u0 + ul].rec : 0;          // (PERREC) the unit's row of the threshold tables
         const int t0 = run * a.run;
         const int t1 = min(t0 + a.run, ROWS ? a.units[g.u0 + ul].T : g.T);
         float mx[ROWMAX ? kFW : 1];
@@ -555,8 +569,8 @@ __global__ void __launch_bounds__(kThreads, B200_K1_MINBLOCKS) k1_analyze(const 
                 const float PB = fmaf(br, br, bi * bi);
                 const int k = lane + 32 * q;
                 const bool valid = (q < 16) || (lane == 0);
-                const float th = s_thr4[k];
-                const float gg = fmaf(s_gco[k], S, th * 8.0e-7f);
+                const float th = PERREC ? __ldg(a.tb.thr4 + rec * kFPad + k) : s_thr4[k];
+                const float gg = fmaf(PERREC ? __ldg(a.tb.gco + rec * kFPad + k) : s_gco[k], S, th * 8.0e-7f);
                 const float dA = PA - th, dB = PB - th;
                 const unsigned wA = __ballot_sync(0xffffffffu, valid && (dA > 0.f));
                 const unsigned wB = __ballot_sync(0xffffffffu, valid && vb && (dB > 0.f));
@@ -601,7 +615,8 @@ __global__ void __launch_bounds__(kThreads, B200_K1_MINBLOCKS) k1_analyze(const 
                             const int src = __ffs((int)m) - 1;
                             m &= m - 1;
                             const int r = recheck_bin_fp64(xrow, base + (long long)fr * H, i1, Lp_u, n_u,
-                                                           src + 32 * q, a.tb.wa64, a.tb.cs64, a.tb.thr2_64, lane);
+                                                           src + 32 * q, a.tb.wa64, a.tb.cs64,
+                                                           PERREC ? a.tb.thr2_64 + rec * kF : a.tb.thr2_64, lane);
                             ++nre;
                             if (r == 0) { ++nun; continue; }
                             if (lane == q) {
@@ -628,7 +643,8 @@ __global__ void __launch_bounds__(kThreads, B200_K1_MINBLOCKS) k1_analyze(const 
             for (int q = 0; q < kFW; ++q)
                 if ((q < 16) || (lane == 0))
                     atomicMax(a.rowmax + (long long)ul * kFPad + lane + 32 * q, __float_as_uint(mx[q]));
-        } else if (4.0f * (float)kN * emax >= 0.999f * a.min_floor4 && lane == 0) {
+        } else if (4.0f * (float)kN * emax >=
+                       0.999f * (PERREC ? __ldg(a.tb.floor4 + rec * kFPad + kFPad - 1) : a.min_floor4) && lane == 0) {
             atomicOr(a.need_rowmax, 1u);             // |X|^2 <= N * (frame energy): a bin could reach its top_db floor
         }
     }
@@ -638,11 +654,9 @@ __global__ void __launch_bounds__(kThreads, B200_K1_MINBLOCKS) k1_analyze(const 
 // top_db floor (spectralgate/utils.py:16): clamped dB > thresh  <=>  raw > thresh  OR
 // (row max over the chunk's frames - top_db > thresh).  One thread per (unit, mask word).
 // =============================================================================================
-__global__ void k_rowfloor(int n_units, const unsigned* __restrict__ rowmax, const float* __restrict__ floor4,
-                           unsigned* __restrict__ rowflag, Counters* cnt) {
-    const int i = blockIdx.x * blockDim.x + threadIdx.x;
-    if (i >= n_units * kFW) return;
-    const int ul = i / kFW, w = i - ul * kFW;
+__device__ __forceinline__ void rowfloor_word(int i, int ul, int w, const unsigned* __restrict__ rowmax,
+                                              const float* __restrict__ floor4, unsigned* __restrict__ rowflag,
+                                              Counters* cnt) {
     unsigned word = 0u, nflag = 0u, namb = 0u;
     for (int b = 0; b < 32; ++b) {
         const int f = w * 32 + b;
@@ -655,6 +669,21 @@ __global__ void k_rowfloor(int n_units, const unsigned* __restrict__ rowmax, con
     rowflag[i] = word;
     if (nflag) atomicAdd(&cnt->floor_flags, (unsigned long long)nflag);
     if (namb) atomicAdd(&cnt->floor_ambiguous, (unsigned long long)namb);
+}
+__global__ void k_rowfloor(int n_units, const unsigned* __restrict__ rowmax, const float* __restrict__ floor4,
+                           unsigned* __restrict__ rowflag, Counters* cnt) {
+    const int i = blockIdx.x * blockDim.x + threadIdx.x;
+    if (i >= n_units * kFW) return;
+    const int ul = i / kFW, w = i - ul * kFW;
+    rowfloor_word(i, ul, w, rowmax, floor4, rowflag, cnt);
+}
+// per-recording thresholds: unit ul (units = the batch's first entry of the unit table) reads its recording's floor4 row
+__global__ void k_rowfloor_rec(int n_units, const UnitDesc* __restrict__ units, const unsigned* __restrict__ rowmax,
+                               const float* __restrict__ floor4, unsigned* __restrict__ rowflag, Counters* cnt) {
+    const int i = blockIdx.x * blockDim.x + threadIdx.x;
+    if (i >= n_units * kFW) return;
+    const int ul = i / kFW, w = i - ul * kFW;
+    rowfloor_word(i, ul, w, rowmax, floor4 + (long long)units[ul].rec * kFPad, rowflag, cnt);
 }
 
 // =============================================================================================
@@ -1910,13 +1939,13 @@ struct K0Args {
     double eps;
     double* db;            // [Tn][F]
 };
-__global__ void __launch_bounds__(256) k0_stft_db(const K0Args a) {
-    B200_DYN_SMEM(double2, s);                      // [N]
-    const int t = blockIdx.x;
+// frame t of the clip yn[0, n) into db[t][F] (the body of k0_stft_db and k0_stft_db_rows)
+__device__ __forceinline__ void k0_stft_db_frame(const K0Args& a, const double* yn, long long n_yn, int t, double* db,
+                                                 double2* s) {
     const long long base = (long long)t * a.H - kN / 2;
     for (int n = threadIdx.x; n < kN; n += blockDim.x) {
         const long long j = base + n;
-        const double v = (j >= 0 && j < a.n) ? a.yn[j] * a.wa64[n] : 0.0;
+        const double v = (j >= 0 && j < n_yn) ? yn[j] * a.wa64[n] : 0.0;
         int r = 0;
         for (int b = 0; b < 10; ++b) r |= ((n >> b) & 1) << (9 - b);
         s[r] = make_double2(v, 0.0);
@@ -1937,16 +1966,57 @@ __global__ void __launch_bounds__(256) k0_stft_db(const K0Args a) {
     }
     for (int f = threadIdx.x; f < kF; f += blockDim.x) {
         const double2 v = s[f];
-        a.db[(long long)t * kF + f] = 20.0 * log10(sqrt(v.x * v.x + v.y * v.y) + a.eps);
+        db[(long long)t * kF + f] = 20.0 * log10(sqrt(v.x * v.x + v.y * v.y) + a.eps);
+    }
+}
+__global__ void __launch_bounds__(256) k0_stft_db(const K0Args a) {
+    B200_DYN_SMEM(double2, s);                      // [N]
+    k0_stft_db_frame(a, a.yn, a.n, blockIdx.x, a.db, s);
+}
+
+// b200gate_noise_stats_rows: a group of clips, each with its own length and frame count, in one launch of each kernel
+struct K0Clip {
+    const void* x;          // sample 0 of channel 0: the clip's samples (device clips) or its channel sums (host clips)
+    long long stride;       // elements between channels
+    long long c_sum;        // channels summed here: C (device clips), 1 (host clips, summed on the host in channel order)
+    long long C;            // channels of the clip: the divisor of the mean
+    long long n;            // samples after clipping
+    long long yn_off;       // offset of its float64 mean in the group's buffer
+    long long t_off;        // its frames are rows [t_off, t_off + Tn) of the group's dB buffer
+    int Tn;                 // n / H + 1
+};
+
+// channel sum in channel order and mean in the accumulation dtype (k0_channel_sum + k0_mean_to_f64); grid.y = clip
+template <typename Tin, typename Tacc>
+__global__ void k0_clip_mean_rows(const K0Clip* __restrict__ clips, double* __restrict__ yn) {
+    const K0Clip c = clips[blockIdx.y];
+    const Tin* y = static_cast<const Tin*>(c.x);
+    for (long long i = (long long)blockIdx.x * blockDim.x + threadIdx.x; i < c.n;
+         i += (long long)gridDim.x * blockDim.x) {
+        Tacc s = (Tacc)0;
+        for (long long ch = 0; ch < c.c_sum; ++ch) s = s + (Tacc)y[ch * c.stride + i];
+        yn[c.yn_off + i] = (double)(s / (Tacc)c.C);
     }
 }
 
-// One CTA per bin: top_db floor, mean, std (ddof), thresh.
-__global__ void __launch_bounds__(256) k0_stats(const double* __restrict__ db, int Tn, int F, double top_db, int ddof,
-                                                double n_std, double* __restrict__ mean_out,
-                                                double* __restrict__ std_out, double* __restrict__ thr_out) {
+// one CTA per frame of the group (blockIdx.x: row of the group's dB buffer), as k0_stft_db per clip
+__global__ void __launch_bounds__(256) k0_stft_db_rows(const K0Args a, const K0Clip* __restrict__ clips, int n_clips) {
+    B200_DYN_SMEM(double2, s);                      // [N]
+    const int t = blockIdx.x;
+    int lo = 0, hi = n_clips - 1;                   // the clip whose frames hold row t
+    while (lo < hi) {
+        const int mid = (lo + hi + 1) >> 1;
+        if (clips[mid].t_off <= t) lo = mid; else hi = mid - 1;
+    }
+    const K0Clip& c = clips[lo];
+    k0_stft_db_frame(a, a.yn + c.yn_off, c.n, t - (int)c.t_off, a.db + c.t_off * kF, s);
+}
+
+// One CTA per bin: top_db floor, mean, std (ddof), thresh (the body of k0_stats and k0_stats_rows).
+__device__ __forceinline__ void k0_stats_bin(const double* __restrict__ db, int Tn, int F, int f, double top_db, int ddof,
+                                             double n_std, double* __restrict__ mean_out, double* __restrict__ std_out,
+                                             double* __restrict__ thr_out) {
     __shared__ double red[256];
-    const int f = blockIdx.x;
     double m = -1.0e300;
     for (int t = threadIdx.x; t < Tn; t += blockDim.x) m = fmax(m, db[(long long)t * F + f]);
     red[threadIdx.x] = m;
@@ -1984,6 +2054,18 @@ __global__ void __launch_bounds__(256) k0_stats(const double* __restrict__ db, i
         std_out[f] = sd;
         thr_out[f] = mean + sd * n_std;
     }
+}
+__global__ void __launch_bounds__(256) k0_stats(const double* __restrict__ db, int Tn, int F, double top_db, int ddof,
+                                                double n_std, double* __restrict__ mean_out,
+                                                double* __restrict__ std_out, double* __restrict__ thr_out) {
+    k0_stats_bin(db, Tn, F, blockIdx.x, top_db, ddof, n_std, mean_out, std_out, thr_out);
+}
+// grid (F, clips): clip blockIdx.y of the group; res holds [clips][3][F] (mean, std, thresh)
+__global__ void __launch_bounds__(256) k0_stats_rows(const double* __restrict__ db, const K0Clip* __restrict__ clips,
+                                                     double top_db, int ddof, double n_std, double* __restrict__ res) {
+    const K0Clip& c = clips[blockIdx.y];
+    double* r = res + (long long)blockIdx.y * 3 * kF;
+    k0_stats_bin(db + c.t_off * kF, c.Tn, kF, blockIdx.x, top_db, ddof, n_std, r, r + kF, r + 2 * kF);
 }
 
 }  // namespace b200
