@@ -313,6 +313,26 @@ int b200gate_stream_push(b200gate_handle* h, const void* in, int64_t n, int64_t 
 int b200gate_stream_finish(b200gate_handle* h, void* out, int64_t out_stride, int64_t out_capacity,
                            int64_t* n_out, void* cuda_stream);
 
+/* ---- TorchGate.stream(): the non-stationary TorchGate on rows that arrive block by block ---------------------------
+ * For a B200GATE_SURFACE_TORCH handle with stationary = 0 at n_fft = win_length = 1024, hop_length = 256 (any other
+ * handle: B200GATE_ERR_STATE).  Every stage of that gate looks ahead a bounded distance, so after R samples per row
+ *     hb(R) = 2 floor(nS / 2),  nS = 2 floor(c / 2) - 1 - right - n_grad_time,  c = floor((R - 512) / 256) + 1
+ * (right = n_movemean - 1 - (n_movemean - 1) / 2) and the samples [0, 256 max(0, hb(R) - 2)) of every row are final.
+ * The concatenation of everything a stream returns is bit-identical to b200gate_run on the concatenated rows.
+ * b200gate_tstream_begin starts (or restarts) a stream of n_rows rows; its device state depends on n_rows and the
+ * parameters only.  b200gate_tstream_push appends samples [0, n) of each row of `in` (device float32 rows, stride
+ * in_stride) and writes the *n_out samples that became final to out[b][0, *n_out) (stride out_stride); it only enqueues
+ * on cuda_stream.  b200gate_tstream_finish writes the rest of the (R / 256) 256 samples and closes the stream (it frees the
+ * stream's device state, which waits for the device).  Errors: out_capacity below what the call returns: B200GATE_ERR_ARG,
+ * the stream unchanged; finish with R < 2 win_length: B200GATE_ERR_ARG ("x must be bigger than 2048"), the stream stays
+ * open.  While a torch stream is open b200gate_run, b200gate_run_rows, b200gate_torch_apply_masks(_rows) and
+ * b200gate_stream_* return B200GATE_ERR_STATE. */
+int b200gate_tstream_begin(b200gate_handle* h, int64_t n_rows);
+int b200gate_tstream_push(b200gate_handle* h, const float* in, int64_t n, int64_t in_stride, float* out, int64_t out_stride,
+                          int64_t out_capacity, int64_t* n_out, void* cuda_stream);
+int b200gate_tstream_finish(b200gate_handle* h, float* out, int64_t out_stride, int64_t out_capacity, int64_t* n_out,
+                            void* cuda_stream);
+
 int b200gate_get_stats(const b200gate_handle* h, b200gate_stats* out);
 
 /* ---- sample formats of device-resident callers ----------------------------------------------------------------------

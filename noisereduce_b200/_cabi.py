@@ -39,6 +39,7 @@ EXPORTS = [
     "b200gate_stream_begin", "b200gate_stream_push", "b200gate_stream_finish", "b200gate_convert",
     "b200gate_mask_store_bytes", "b200gate_set_mask_store", "b200gate_adjoint", "b200gate_run_rows",
     "b200gate_torch_apply_masks_rows", "b200gate_noise_stats_rows", "b200gate_set_noise_threshold_rows",
+    "b200gate_tstream_begin", "b200gate_tstream_push", "b200gate_tstream_finish",
 ]
 
 
@@ -146,6 +147,9 @@ class GateLibrary:
         d.b200gate_torch_apply_masks_rows.argtypes = [vp, C.POINTER(Row), i64, C.c_int, C.c_int, vp]
         d.b200gate_noise_stats_rows.argtypes = [vp, C.POINTER(NoiseClip), i64, C.c_int, C.c_int, C.POINTER(dbl), vp]
         d.b200gate_set_noise_threshold_rows.argtypes = [vp, C.POINTER(dbl), i64, i32]
+        d.b200gate_tstream_begin.argtypes = [vp, i64]
+        d.b200gate_tstream_push.argtypes = [vp, vp, i64, i64, vp, i64, i64, C.POINTER(i64), vp]
+        d.b200gate_tstream_finish.argtypes = [vp, vp, i64, i64, C.POINTER(i64), vp]
 
 
 def format_code(dt) -> int:
@@ -401,6 +405,21 @@ class Gate:
     def stream_finish(self, out_ptr, out_stride, out_capacity, stream=None) -> int:
         n_out = C.c_int64()
         self._check(self.lib.dll.b200gate_stream_finish(self._h, out_ptr, out_stride, out_capacity, C.byref(n_out), stream))
+        return n_out.value
+
+    # -- torch streams (b200gate_tstream_*): device float32 rows; the push / finish return n_out -------------------------
+    def tstream_begin(self, n_rows):
+        self._check(self.lib.dll.b200gate_tstream_begin(self._h, n_rows))
+
+    def tstream_push(self, in_ptr, n, in_stride, out_ptr, out_stride, out_capacity, stream=None) -> int:
+        n_out = C.c_int64()
+        self._check(self.lib.dll.b200gate_tstream_push(self._h, in_ptr, n, in_stride, out_ptr, out_stride, out_capacity,
+                                                       C.byref(n_out), stream))
+        return n_out.value
+
+    def tstream_finish(self, out_ptr, out_stride, out_capacity, stream=None) -> int:
+        n_out = C.c_int64()
+        self._check(self.lib.dll.b200gate_tstream_finish(self._h, out_ptr, out_stride, out_capacity, C.byref(n_out), stream))
         return n_out.value
 
     def set_range(self, mode: int, a: int = 0, b: int = 0):

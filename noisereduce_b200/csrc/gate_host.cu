@@ -21,6 +21,7 @@
 #include <string.h>
 
 #include <algorithm>
+#include <climits>
 #include <condition_variable>
 #include <functional>
 #include <future>
@@ -37,6 +38,7 @@ const double kEps64 = 2.220446049250313e-16;       // np.finfo(np.float64).eps (
 const double kEps32 = 5.9604644775390625e-08;      // 2^-24, FP32 unit roundoff
 const double kKappa = 16.0;                        // guard band: |dX| <= kappa * eps32 * ||frame pair||_2
 thread_local std::string g_create_error;          // one handle per thread: a failed create reports through the calling thread
+const char* const kTsOpen = "a torch stream is open on this handle (b200gate_tstream_finish first)";
 
 }  // namespace
 
@@ -124,6 +126,18 @@ struct b200gate_handle {
     long long s_cap = 0, s_slice = 0, s_ocap = 0;  // window pitch, samples one slice appends at most, output pitch
     void *d_swin = nullptr, *d_sout = nullptr;
     size_t swin_bytes = 0, sout_bytes = 0;
+    // TorchGate.stream() (b200gate_tstream_*): ts_B rows advancing together; ts_R samples received per row.  Frames
+    // [0, ts_nA) have |X| and spectra, [0, ts_nM) the moving-mean mask, [0, ts_nS) the final mask; hops [2, ts_ha) have
+    // been returned.  One device allocation holds the sample window [ts_lo, ts_R) (row pitch ts_cap) and the frame
+    // rings of ts_ring frames (StreamWin); see b200gate_tstream_begin.
+    bool ts_open = false;
+    long long ts_B = 0, ts_R = 0, ts_lo = 0, ts_cap = 0, ts_slice = 0;
+    long long ts_nA = 0, ts_nM = 0, ts_nS = 0, ts_ha = 2;
+    int ts_ring = 0;
+    void* d_ts = nullptr;
+    float *d_ts_win = nullptr, *d_ts_mag = nullptr, *d_ts_m0 = nullptr, *d_ts_mask = nullptr;
+    float2* d_ts_z = nullptr;
+    double* d_ts_run = nullptr;
     // b200gate_run_rows: the call's unit table, written by the host into hp_units and copied to d_units on the call's
     // stream; ev_units marks that copy, so the next call can rewrite hp_units without waiting for the device
     UnitDesc* hp_units = nullptr;
@@ -772,10 +786,10 @@ static void launch_stationary_numerators(const b200gate_handle* h, const SmoothA
 
 // Float-mask smoothing (non-stationary gate, TorchGate moving-mean gate): the box form for 1 <= nf <= 12 (k_smooth_box,
 // compiled per nf), else the tap-loop streaming kernel, else (ring too large for shared memory) the tile kernel.
-#define B200_SMOOTH_BOX_CASE(NF_) case NF_: { auto kern_ = ROWS ? k_smooth_box<NF_, true> : k_smooth_box<NF_>; \
+#define B200_SMOOTH_BOX_CASE(NF_) case NF_: { auto kern_ = k_smooth_box<NF_, ROWS, STREAM>; \
         if (set_attr) cudaFuncSetAttribute(kern_, cudaFuncAttributeMaxDynamicSharedMemorySize, 200 * 1024); \
         else B200_LAUNCH(kern_, grid, dim3(sa.FPad / 4), smem, st, sa); } break;
-template <bool ROWS = false>
+template <bool ROWS = false, bool STREAM = false>
 static void smooth_box_dispatch(const SmoothFArgs& sa, int nf, dim3 grid, size_t smem, cudaStream_t st, bool set_attr) {
     switch (nf) {
         B200_SMOOTH_BOX_CASE(1) B200_SMOOTH_BOX_CASE(2) B200_SMOOTH_BOX_CASE(3) B200_SMOOTH_BOX_CASE(4)
@@ -784,21 +798,22 @@ static void smooth_box_dispatch(const SmoothFArgs& sa, int nf, dim3 grid, size_t
         default: break;
     }
 }
-// ROWS (b200gate_run_rows; sa.units set, tf_hi the largest of the batch): the two streaming kernels only -- false when the
-// ring does not fit shared memory.
-template <bool ROWS = false>
+// ROWS (b200gate_run_rows; sa.units set, tf_hi the largest of the batch) and STREAM (b200gate_tstream_*; sa.sw set): the
+// two streaming kernels only -- false when the ring does not fit shared memory.
+template <bool ROWS = false, bool STREAM = false>
 static bool launch_smooth_float(SmoothFArgs sa, int nf, int nt, int tf_lo, int tf_hi, int nu, int path_flags, cudaStream_t st) {
     const bool box_ok = nf >= 1 && nf <= 12 && sa.FPad - sa.F >= 12 && smoothb_smem_bytes(sa.FPad, nt) <= 200 * 1024 &&
                         !(path_flags & 32) && !(path_flags & 128);
     if (box_ok) {
         sa.TT = 256;                        // frames per strip (2 nt warm-up rows each)
         const int strips = (tf_hi - tf_lo + sa.TT - 1) / sa.TT;
-        smooth_box_dispatch<ROWS>(sa, nf, dim3(strips, nu), smoothb_smem_bytes(sa.FPad, nt), st, false);
+        smooth_box_dispatch<ROWS, STREAM>(sa, nf, dim3(strips, nu), smoothb_smem_bytes(sa.FPad, nt), st, false);
     } else if (smooths_smem_bytes(sa.FPad, nf, nt) <= 200 * 1024 && !(path_flags & 32)) {
         sa.TT = 256;
         const int strips = (tf_hi - tf_lo + sa.TT - 1) / sa.TT;
-        B200_LAUNCH(k_smooth_stream<ROWS>, dim3(strips, nu), dim3(sa.FPad / 4), smooths_smem_bytes(sa.FPad, nf, nt), st, sa);
-    } else if (ROWS) {
+        auto kern_ = k_smooth_stream<ROWS, STREAM>;
+        B200_LAUNCH(kern_, dim3(strips, nu), dim3(sa.FPad / 4), smooths_smem_bytes(sa.FPad, nf, nt), st, sa);
+    } else if (ROWS || STREAM) {
         return false;
     } else {
         const int tiles = (tf_hi - tf_lo + sa.TT - 1) / sa.TT;
@@ -1045,6 +1060,12 @@ int b200gate_create(const b200gate_params* p, b200gate_handle** out) {
         for (int nfb = 1; nfb <= 12; ++nfb) smooth_box_dispatch<true>(SmoothFArgs{}, nfb, dim3(1), 0, nullptr, true);
         // (torch surface, stationary extents beyond the in-synthesis smoothing: numerators from k_smooth_generic)
         cudaFuncSetAttribute(k_smooth_generic<true>, cudaFuncAttributeMaxDynamicSharedMemorySize, 160 * 1024);
+        // b200gate_tstream_*: the STREAM instantiations
+        cudaFuncSetAttribute(k1n_magnitude<8, float, false, true>, cudaFuncAttributeMaxDynamicSharedMemorySize, k1n_smem_floats() * 4);
+        cudaFuncSetAttribute(k2c_synthesize<8, kMaskF32, float, false, true>, cudaFuncAttributeMaxDynamicSharedMemorySize,
+                             k2c_smem_bytes<kMaskF32>());
+        cudaFuncSetAttribute(k_smooth_stream<false, true>, cudaFuncAttributeMaxDynamicSharedMemorySize, 200 * 1024);
+        for (int nfb = 1; nfb <= 12; ++nfb) smooth_box_dispatch<false, true>(SmoothFArgs{}, nfb, dim3(1), 0, nullptr, true);
         cudaFuncSetAttribute(k2c_synthesize<8, kMaskU16, float, true>, cudaFuncAttributeMaxDynamicSharedMemorySize, k2c_smem_bytes<kMaskU16>());
         cudaFuncSetAttribute(k2c_synthesize<8, kMaskU16Blend, float, true>, cudaFuncAttributeMaxDynamicSharedMemorySize, k2c_smem_bytes<kMaskU16Blend>());
         cudaFuncSetAttribute(k1n_magnitude_2k, cudaFuncAttributeMaxDynamicSharedMemorySize, k1n2_smem_floats() * 4);
@@ -1100,6 +1121,7 @@ void b200gate_destroy(b200gate_handle* h) {
     g_pinned_pool.give(h->hp_units, h->hp_units_bytes);
     if (h->d_units) cudaFree(h->d_units);
     if (h->d_rtab) cudaFree(h->d_rtab);
+    if (h->d_ts) cudaFree(h->d_ts);
     if (h->ev_units) cudaEventDestroy(h->ev_units);
     for (cudaEvent_t e : h->stage_ev) cudaEventDestroy(e);
     for (cudaEvent_t e : h->pipe_ev) cudaEventDestroy(e);
@@ -2584,6 +2606,7 @@ static int run_core(b200gate_handle* h, const void* in, void* out, int dtype, in
 int b200gate_run(b200gate_handle* h, const void* in, void* out, int dtype, int64_t C, int64_t N, int64_t in_stride,
                  int64_t out_stride, int is_device, void* stream) {
     if (h && h->s_open) return fail(h, B200GATE_ERR_STATE, "a stream is open on this handle (b200gate_stream_finish first)");
+    if (h && h->ts_open) return fail(h, B200GATE_ERR_STATE, kTsOpen);
     if (h) h->keep_masks = h->mask_store != nullptr;
     const int rc = run_core(h, in, out, dtype, C, N, in_stride, out_stride, is_device, stream, 0);
     if (h) h->keep_masks = false;
@@ -2598,6 +2621,7 @@ int b200gate_run(b200gate_handle* h, const void* in, void* out, int dtype, int64
 int b200gate_run_rows(b200gate_handle* h, const b200gate_row* rows, int64_t n_rows, int dtype, int is_device, void* stream) {
     if (!h || !rows || n_rows <= 0 || dtype_size(dtype) == 0) return fail(h, B200GATE_ERR_ARG, "bad argument");
     if (h->s_open) return fail(h, B200GATE_ERR_STATE, "a stream is open on this handle (b200gate_stream_finish first)");
+    if (h->ts_open) return fail(h, B200GATE_ERR_STATE, kTsOpen);
     const b200gate_params& p = h->p;
     // torch: TorchGate.forward on each row (one unit per row: no chunk grid, no padding, torch.istft output length)
     const bool torch = p.surface == B200GATE_SURFACE_TORCH;
@@ -3299,6 +3323,7 @@ bool stream_needs_thresholds(const b200gate_handle* h) {
 }
 
 int stream_check_space(b200gate_handle* h, int is_device) {
+    if (h->ts_open) return fail(h, B200GATE_ERR_STATE, kTsOpen);
     if (!h->s_open) return fail(h, B200GATE_ERR_STATE, "no open stream (b200gate_stream_begin first)");
     if (h->s_is_device >= 0 && h->s_is_device != (is_device ? 1 : 0))
         return fail(h, B200GATE_ERR_ARG, "every push of a stream must use the same memory space (is_device)");
@@ -3309,6 +3334,7 @@ int stream_check_space(b200gate_handle* h, int is_device) {
 
 int b200gate_stream_begin(b200gate_handle* h, int dtype, int64_t C) {
     if (!h) return B200GATE_ERR_ARG;
+    if (h->ts_open) return fail(h, B200GATE_ERR_STATE, kTsOpen);
     h->s_open = false;
     if (h->p.surface == B200GATE_SURFACE_TORCH)
         return fail(h, B200GATE_ERR_ARG, "streaming needs the numpy or the chunked torch surface");
@@ -3420,9 +3446,213 @@ int b200gate_stream_finish(b200gate_handle* h, void* out, int64_t out_stride, in
 }
 
 
+// ---- TorchGate.stream(): the non-stationary TorchGate on rows that arrive block by block ------------------------------
+// Every stage of the gate looks ahead a bounded number of frames: frame t of torch.stft(center=True) needs samples up to
+// t H + n_fft / 2, the moving mean of frame t needs |X| up to frame t + right, the smoothing of frame t masks up to t + nt,
+// and the overlap-add of hop h frames h - 3 .. h.  So after R samples per row the stream can finish
+//   nA(R) = 2 floor(c / 2) frames of analysis, c = floor((R - n_fft / 2) / H) + 1 (the frames whose samples are in),
+//   nM = nA - 1 - right frames of moving mean, nS = nM - nt frames of smoothing,
+//   hops [2, hb), hb = 2 floor(nS / 2): output samples [0, (hb - 2) H)
+// (each clamped at 0).  Frames are analysed and synthesised in the global pairs (2j, 2j+1) of b200gate_run, the moving
+// mean carries its double running sum per (row, bin), and the smoothing restarts in every frame, so every returned sample
+// equals b200gate_run on the whole rows in every bit; b200gate_tstream_finish does the last frames with T = R / H + 1.
+namespace {
+
+long long ts_hops_done(const b200gate_handle* h, long long R) {      // hb(R) above
+    const int n = h->p.n_movemean, right = n - 1 - (n - 1) / 2;
+    if (R < kN / 2) return 2;
+    const long long c = (R - kN / 2) / h->p.hop_length + 1;
+    const long long nS = (c & ~1LL) - 1 - right - h->p.n_grad_time;
+    return std::max(2LL, nS & ~1LL);
+}
+
+// Advance the stream to R = h->ts_R received samples (T = 0) or to its end (T = R / H + 1 frames): analysis, moving mean,
+// smoothing, synthesis of what has become final.  The hops returned go to out[b][0, ...) (row stride out_stride).
+int ts_advance(b200gate_handle* h, long long T, float* out, long long out_stride, cudaStream_t st) {
+    const b200gate_params& p = h->p;
+    const int H = p.hop_length, nt = p.n_grad_time, nf = p.n_grad_freq, ring = h->ts_ring;
+    const int n = p.n_movemean, right = n - 1 - (n - 1) / 2;
+    const int B = (int)h->ts_B;
+    const bool fin = T > 0;
+    const int Tb = fin ? (int)T : INT_MAX;                   // the frame bound the kernels see
+    const long long R = h->ts_R;
+    const long long c = R >= kN / 2 ? (R - kN / 2) / H + 1 : 0;
+    const long long nA = fin ? T : (c & ~1LL);
+    const long long nM = fin ? T : std::max(h->ts_nM, nA - 1 - right);
+    const long long nS = fin ? T : std::max(h->ts_nS, nM - nt);
+    const long long hb = fin ? T + 1 : std::max(h->ts_ha, nS & ~1LL);
+    const Tables tb = device_tables(h);
+    StreamWin sw{};
+    sw.ring = ring;
+    if (nA > h->ts_nA) {
+        K1nArgs a1{};
+        a1.g.H = H; a1.g.C = B; a1.g.T = (int)nA; a1.g.n_chunks = 1; a1.g.n_total = R; a1.g.step = R; a1.g.pad = 0;
+        a1.g.Lp = R; a1.g.in_stride = h->ts_cap; a1.g.u0 = 0; a1.g.n_units = B;
+        a1.tb = tb; a1.x = h->d_ts_win - h->ts_lo; a1.mag = h->d_ts_mag; a1.dbg.ul = -1; a1.zcache = h->d_ts_z;
+        a1.zpairs = ring / 2; a1.z_lo = 0; a1.z_hi = INT_MAX;
+        sw.f0 = (int)h->ts_nA;
+        a1.sw = sw;
+        a1.run = 2;                                           // one frame pair per work item (pairs are global either way)
+        a1.n_runs = (int)((nA - h->ts_nA + 1) / 2);
+        auto kern_ = k1n_magnitude<8, float, false, true>;
+        B200_LAUNCH(kern_, dim3(grid_1d((long long)B * a1.n_runs, kWarps, h->num_sm * 3)), dim3(kThreads),
+                    k1n_smem_floats() * 4, st, a1);
+    }
+    if (nM > h->ts_nM) {
+        TMovArgs ma{};
+        ma.n_units = B; ma.T = Tb; ma.n_movemean = n; ma.n_thresh = (float)p.thresh_n_mult;
+        ma.inv_temp = (float)p.sigmoid_slope; ma.p = (float)p.prop_decrease; ma.mag = h->d_ts_mag; ma.m0 = h->d_ts_m0;
+        sw.f0 = (int)h->ts_nM;
+        ma.sw = sw; ma.f1 = (int)nM; ma.run = h->d_ts_run;
+        auto kern_ = k_tgate_movmean<false, true>;
+        B200_LAUNCH(kern_, dim3(grid_1d((long long)B * kFPad, 128, 1 << 30)), dim3(128), 0, st, ma);
+    }
+    if (nS > h->ts_nS) {
+        SmoothFArgs sa{};
+        sa.n_units = B; sa.T = Tb; sa.nf = nf; sa.nt = nt; sa.tf_lo = (int)h->ts_nS; sa.tf_hi = (int)nS; sa.F = kF; sa.FPad = kFPad;
+        sa.p = 1.0f; sa.one_minus_p = 0.0f;                  // (the torch surface blends in k_tgate_movmean)
+        sa.m0 = h->d_ts_m0; sa.m2 = h->d_ts_mask; sa.sw = sw;
+        launch_smooth_float<false, true>(sa, nf, nt, (int)h->ts_nS, (int)nS, B, 0, st);   // (extents checked at begin)
+    }
+    if (hb > h->ts_ha) {
+        // hops [ha, hb): Geom's padded-chunk view with pad = (ha - 2) H puts the first of them at h_lo and output sample
+        // (ha - 2) H at out[b][0]; while the end is unknown, T = hb + 1 keeps every hop interior
+        const long long P = (h->ts_ha - 2) * H;
+        const long long out_len = (fin ? (T - 1) * H : (hb - 2) * H) - P;
+        K2Args a2{};
+        a2.g.H = H; a2.g.C = B; a2.g.T = fin ? (int)T : (int)hb + 1; a2.g.n_chunks = 1; a2.g.n_total = out_len;
+        a2.g.step = out_len; a2.g.pad = P; a2.g.Lp = out_len + P; a2.g.out_stride = out_stride; a2.g.u0 = 0; a2.g.n_units = B;
+        a2.tb = tb; a2.y = out; a2.fmask = h->d_ts_mask; a2.zcache = h->d_ts_z; a2.zpairs = ring / 2; a2.nt = nt;
+        a2.dbg.ul = -1; a2.sw = sw;
+        const long long hops = hb - h->ts_ha;
+        long long want = (long long)h->num_sm * 3 * kWarps * 4;
+        long long run = std::max(16LL, std::min(128LL, ((long long)B * hops + want - 1) / want));
+        run += run & 1;                                       // work items end on odd frames, as in b200gate_run
+        a2.run = (int)run;
+        a2.n_runs = (int)((hops + run - 1) / run);
+        auto kern_ = k2c_synthesize<8, kMaskF32, float, false, true>;
+        B200_LAUNCH(kern_, dim3(grid_1d((long long)B * a2.n_runs, kWarps, h->num_sm * 3)), dim3(kThreads),
+                    k2c_smem_bytes<kMaskF32>(), st, a2);
+    }
+    CK(h, cudaGetLastError());
+    h->ts_nA = nA; h->ts_nM = nM; h->ts_nS = nS; h->ts_ha = hb;
+    return B200GATE_OK;
+}
+
+void ts_release(b200gate_handle* h) {
+    if (h->d_ts) cudaFree(h->d_ts);
+    h->d_ts = nullptr;
+    h->ts_open = false;
+}
+
+}  // namespace
+
+int b200gate_tstream_begin(b200gate_handle* h, int64_t n_rows) {
+    if (!h) return B200GATE_ERR_ARG;
+    const b200gate_params& p = h->p;
+    if (p.surface != B200GATE_SURFACE_TORCH || p.stationary || h->generic || p.n_fft != kN || p.win_length != kN ||
+        p.hop_length != 256)
+        return fail(h, B200GATE_ERR_STATE, "torch streams need a non-stationary TORCH-surface handle at n_fft = win_length "
+                    "= 1024, hop_length = 256 (the stationary gate's statistics span the whole row)");
+    if (h->s_open) return fail(h, B200GATE_ERR_STATE, "a stream is open on this handle (b200gate_stream_finish first)");
+    if (n_rows <= 0 || n_rows > 0x7fffffffLL / kFPad) return fail(h, B200GATE_ERR_ARG, "bad argument");
+    const int nf = p.n_grad_freq, nt = p.n_grad_time;
+    const bool box = nf >= 1 && nf <= 12 && smoothb_smem_bytes(kFPad, nt) <= 200 * 1024;
+    if (!box && smooths_smem_bytes(kFPad, nf, nt) > 200 * 1024)
+        return fail(h, B200GATE_ERR_ARG, "smoothing extents (%d, %d) beyond the shared-memory ring of the streaming smoothing",
+                    nf, nt);
+    ts_release(h);
+    const int n = p.n_movemean, left = (n - 1) / 2, right = n - 1 - left;
+    // A push is consumed in slices of S samples: a slice adds at most S / H + 2 frames to each stage.  Frames live in the
+    // rings from their analysis until the last stage reads them: the moving mean reads |X| from nM - left to nA, the
+    // smoothing masks from nS - nt to nM, the synthesis spectra and masks from hop ha - 4 (<= nS - 5) on.  Between
+    // slices nA - nM <= right + 1 and nM - nS <= nt, so left + right + 2 nt + S / H + 8 frames always suffice.
+    const long long S = 4096;
+    long long need = left + right + 2LL * nt + S / 256 + 16, ring = 16;
+    while (ring < need) ring *= 2;
+    if (ring > (1 << 20)) return fail(h, B200GATE_ERR_ARG, "n_movemean %d: frame rings too large", n);
+    // the sample window keeps [nA H - n_fft / 2, R) (< 2 H + n_fft samples) before a slice; with a pitch of
+    // S + 2 (2 H + n_fft) a compaction never moves a span onto itself
+    const long long cap = S + 2 * (2 * 256 + kN);
+    const size_t B = (size_t)n_rows;
+    auto al = [](size_t v) { return (v + 255) / 256 * 256; };
+    const size_t o_win = 0, o_z = o_win + al(B * cap * 4), o_mag = o_z + al(B * (size_t)(ring / 2) * 1024 * 8);
+    const size_t o_m0 = o_mag + al(B * ring * kFPad * 4), o_mask = o_m0 + al(B * ring * kFPad * 4);
+    const size_t o_run = o_mask + al(B * ring * kFPad * 4), bytes = o_run + al(B * kFPad * 8);
+    cudaError_t e = cudaMalloc(&h->d_ts, bytes);
+    if (e != cudaSuccess) {
+        cudaGetLastError();
+        h->d_ts = nullptr;
+        return fail(h, B200GATE_ERR_NOMEM, "cudaMalloc(%zu bytes) for the torch stream failed: %s", bytes, cudaGetErrorString(e));
+    }
+    char* base = (char*)h->d_ts;
+    h->d_ts_win = (float*)(base + o_win); h->d_ts_z = (float2*)(base + o_z); h->d_ts_mag = (float*)(base + o_mag);
+    h->d_ts_m0 = (float*)(base + o_m0); h->d_ts_mask = (float*)(base + o_mask); h->d_ts_run = (double*)(base + o_run);
+    h->ts_B = n_rows; h->ts_R = 0; h->ts_lo = 0; h->ts_cap = cap; h->ts_slice = S; h->ts_ring = (int)ring;
+    h->ts_nA = 0; h->ts_nM = 0; h->ts_nS = 0; h->ts_ha = 2;
+    h->ts_open = true;
+    return B200GATE_OK;
+}
+
+int b200gate_tstream_push(b200gate_handle* h, const float* in, int64_t n, int64_t in_stride, float* out, int64_t out_stride,
+                          int64_t out_capacity, int64_t* n_out, void* stream) {
+    if (!h) return B200GATE_ERR_ARG;
+    if (!h->ts_open) return fail(h, B200GATE_ERR_STATE, "no open torch stream (b200gate_tstream_begin first)");
+    if (!n_out || n < 0 || (n > 0 && (!in || in_stride < n)) || out_capacity < 0 || (out_capacity > 0 && !out) ||
+        (h->ts_B > 1 && out_stride < out_capacity))
+        return fail(h, B200GATE_ERR_ARG, "bad argument");
+    const long long H = h->p.hop_length;
+    const long long m = (ts_hops_done(h, h->ts_R + n) - h->ts_ha) * H;
+    if (out_capacity < m)
+        return fail(h, B200GATE_ERR_ARG, "out_capacity %lld < %lld samples returned by this push", (long long)out_capacity, m);
+    *n_out = m;
+    if (n == 0) return B200GATE_OK;
+    cudaStream_t st = (cudaStream_t)stream;
+    const long long B = h->ts_B, S = h->ts_slice, ha0 = h->ts_ha;
+    int rc;
+    for (long long off = 0; off < n;) {
+        const long long s = std::min(S, n - off);
+        if (h->ts_R - h->ts_lo + s > h->ts_cap) {            // compact: keep the samples of frames nA on
+            const long long lo = std::max(0LL, h->ts_nA * H - kN / 2), L = h->ts_R - lo;
+            if (L > 0)
+                CK(h, cudaMemcpy2DAsync(h->d_ts_win, (size_t)h->ts_cap * 4, h->d_ts_win + (lo - h->ts_lo), (size_t)h->ts_cap * 4,
+                                        (size_t)L * 4, (size_t)B, cudaMemcpyDeviceToDevice, st));
+            h->ts_lo = lo;
+        }
+        CK(h, cudaMemcpy2DAsync(h->d_ts_win + (h->ts_R - h->ts_lo), (size_t)h->ts_cap * 4, in + off, (size_t)in_stride * 4,
+                                (size_t)s * 4, (size_t)B, cudaMemcpyDeviceToDevice, st));
+        h->ts_R += s;
+        off += s;
+        if ((rc = ts_advance(h, 0, out ? out + (h->ts_ha - ha0) * H : nullptr, out_stride, st))) {
+            ts_release(h);
+            return rc;
+        }
+    }
+    return B200GATE_OK;
+}
+
+int b200gate_tstream_finish(b200gate_handle* h, float* out, int64_t out_stride, int64_t out_capacity, int64_t* n_out,
+                            void* stream) {
+    if (!h) return B200GATE_ERR_ARG;
+    if (!h->ts_open) return fail(h, B200GATE_ERR_STATE, "no open torch stream (b200gate_tstream_begin first)");
+    if (!n_out || out_capacity < 0 || (out_capacity > 0 && !out) || (h->ts_B > 1 && out_stride < out_capacity))
+        return fail(h, B200GATE_ERR_ARG, "bad argument");
+    const long long H = h->p.hop_length, R = h->ts_R;
+    if (R < 2 * h->p.win_length) return fail(h, B200GATE_ERR_ARG, "x must be bigger than %d", 2 * h->p.win_length);
+    const long long T = R / H + 1, m = (T + 1 - h->ts_ha) * H;      // the rest of torch.istft's (T - 1) H samples
+    if (out_capacity < m)
+        return fail(h, B200GATE_ERR_ARG, "out_capacity %lld < %lld samples returned by finish", (long long)out_capacity, m);
+    *n_out = m;
+    const int rc = ts_advance(h, T, out, out_stride, (cudaStream_t)stream);
+    ts_release(h);                                            // (cudaFree waits for the device)
+    return rc;
+}
+
+
 int b200gate_torch_apply_masks(b200gate_handle* h, const void* in, void* out, int dtype, int64_t C, int64_t N, int64_t in_stride,
                                int64_t out_stride, int is_device, void* stream) {
     if (!h) return B200GATE_ERR_ARG;
+    if (h->ts_open) return fail(h, B200GATE_ERR_STATE, kTsOpen);
     if (h->p.surface != B200GATE_SURFACE_TORCH) return fail(h, B200GATE_ERR_STATE, "torch surface only");
     if (!h->masks_valid || h->masks_C != C || h->masks_N != N)
         return fail(h, B200GATE_ERR_STATE, "no masks of a matching forward are kept (run b200gate_run on [%lld][%lld] first; "
@@ -3436,6 +3666,7 @@ int b200gate_torch_apply_masks(b200gate_handle* h, const void* in, void* out, in
 int b200gate_torch_apply_masks_rows(b200gate_handle* h, const b200gate_row* rows, int64_t n_rows, int dtype, int is_device,
                                     void* stream) {
     if (!h) return B200GATE_ERR_ARG;
+    if (h->ts_open) return fail(h, B200GATE_ERR_STATE, kTsOpen);
     if (h->p.surface != B200GATE_SURFACE_TORCH) return fail(h, B200GATE_ERR_STATE, "torch surface only");
     if (!rows || n_rows <= 0) return fail(h, B200GATE_ERR_ARG, "bad argument");
     bool match = h->masks_valid && (int64_t)h->masks_rows_n.size() == n_rows;

@@ -70,6 +70,14 @@ struct UnitDesc {
     int run;                // k2c_synthesize: output hops per work item, as run_core sizes them for this unit's recording
 };
 
+// TorchGate.stream() (b200gate_tstream_*): the kernels templated with STREAM address global frame t of a row in slot
+// t & (ring - 1) of the row's frame rings (|X|, masks: ring rows of FPad floats; spectra: ring / 2 frame pairs), and
+// k1n_magnitude / k_tgate_movmean start at global frame f0.  ring is a power of two, so pairs (2j, 2j+1) are adjacent.
+struct StreamWin {
+    int f0;
+    int ring;
+};
+
 struct Tables {              // device pointers, built once per handle
     const float* wa;         // [N] analysis window / sum(w)
     const float* ws;         // [N] synthesis window * sum(w) / N
@@ -940,6 +948,7 @@ struct K2Args {
     float* adj;
     long long adj_pitch;
     const UnitDesc* units;         // k2c_synthesize<.., ROWS = true>: the call's unit table
+    StreamWin sw;                  // k2c_synthesize<.., STREAM = true>: zcache / fmask are the stream's rings (zpairs = ring / 2)
 };
 
 constexpr int k2_smem_floats(int H) { return 2 * kN + 2 * kN + H + kFPad + kWarps * kExchFloats + 8 + kWarps * 2 * kN; }
@@ -1270,11 +1279,12 @@ struct K1nArgs {
     int zpairs;
     int z_lo, z_hi;
     const UnitDesc* units;     // ROWS instantiations: the call's unit table
+    StreamWin sw;              // STREAM instantiations: frames [sw.f0, g.T) into the rings
 };
 
 constexpr int k1n_smem_floats() { return kN + 2 * kN + kWarps * kExchFloats; }
 
-template <int HR, typename T, bool ROWS = false>
+template <int HR, typename T, bool ROWS = false, bool STREAM = false>
 __global__ void __launch_bounds__(kThreads, 3) k1n_magnitude(const K1nArgs a) {
     B200_DYN_SMEM(float, smem);
     float* s_wa = smem;
@@ -1302,7 +1312,7 @@ __global__ void __launch_bounds__(kThreads, 3) k1n_magnitude(const K1nArgs a) {
         const T* xrow = ROWS ? static_cast<const T*>(d->x) : static_cast<const T*>(a.x) + (long long)c * g.in_stride;
         const long long Lp_u = ROWS ? d->Lp : g.Lp, n_u = ROWS ? d->n_total : g.n_total;
         const int T_u = ROWS ? d->T : g.T;
-        const int t0 = run * a.run;
+        const int t0 = (STREAM ? a.sw.f0 : 0) + run * a.run;
         const int t1 = min(t0 + a.run, T_u);
         for (int t = t0; t < t1; t += 2) {
             const bool vb = (t + 1 < t1);
@@ -1311,12 +1321,14 @@ __global__ void __launch_bounds__(kThreads, 3) k1n_magnitude(const K1nArgs a) {
             load_frame_pair<HR>(re, im, xrow, base, i1, Lp_u, n_u, s_wa, lane, vb);
             warp_fft1024(re, im, tile, s_tw, lane);
             if (a.zcache && t >= a.z_lo && t < a.z_hi) {
-                float2* zp = a.zcache + ((long long)ul * a.zpairs + (t >> 1)) * 1024 + lane;
+                const long long zrow = STREAM ? (long long)ul * (a.sw.ring >> 1) + ((t >> 1) & ((a.sw.ring >> 1) - 1))
+                                              : (long long)ul * a.zpairs + (t >> 1);
+                float2* zp = a.zcache + zrow * 1024 + lane;
 #pragma unroll
                 for (int q = 0; q < 32; ++q) zp[32 * q] = make_float2(re[brev5(q)], im[brev5(q)]);
             }
             if (!a.mag && a.dbg.ul != ul) continue;        // spectra only
-            float* dstA = a.mag + ((long long)ul * g.T + t) * kFPad;
+            float* dstA = a.mag + (STREAM ? (long long)ul * a.sw.ring + (t & (a.sw.ring - 1)) : (long long)ul * g.T + t) * kFPad;
 #pragma unroll
             for (int q = 0; q < kFW; ++q) {
                 const int sA = brev5(q), sP = brev5(31 - q), s0 = brev5((32 - q) & 31);
@@ -1505,6 +1517,7 @@ struct SmoothFArgs {
     float* m2;                 // [n_units][T][FPad]
     const UnitDesc* units;     // ROWS instantiations: units + (first unit of the batch); T is then the pitch only and
                                // tf_hi the largest of the batch
+    StreamWin sw;              // STREAM instantiations: m0 / m2 are rings of sw.ring rows; T bounds the frames only
 };
 __host__ __device__ inline int smoothf_cpitch(int FPad, int nf) { return FPad + 2 * nf + 1; }
 inline size_t smoothf_smem_bytes(int TT, int FPad, int nf) { return (size_t)TT * smoothf_cpitch(FPad, nf) * 4; }
@@ -1555,7 +1568,7 @@ __global__ void __launch_bounds__(256) k_smooth_f(const SmoothFArgs a) {
 // once per strip and written once.
 inline size_t smooths_smem_bytes(int FPad, int nf, int nt) { return ((size_t)(2 * nt + 1) * FPad + FPad + 2 * nf + 8) * 4; }
 
-template <bool ROWS = false>
+template <bool ROWS = false, bool STREAM = false>
 __global__ void __launch_bounds__(288) k_smooth_stream(const SmoothFArgs a) {
     B200_DYN_SMEM(float, s_buf);
     const int FP = a.FPad, FF = a.F, nt = a.nt, nf = a.nf, R = 2 * nt + 1;
@@ -1567,15 +1580,16 @@ __global__ void __launch_bounds__(288) k_smooth_stream(const SmoothFArgs a) {
     const int t_begin = a.tf_lo + blockIdx.x * a.TT;
     if (t_begin >= tf_hi) return;
     const int t_end = min(t_begin + a.TT, tf_hi);
-    const float* src = a.m0 + (long long)ul * a.T * FP;
-    float* dst = a.m2 + (long long)ul * a.T * FP;
+    const int pitch = STREAM ? a.sw.ring : a.T, rmask = STREAM ? a.sw.ring - 1 : -1;    // (row t: t & rmask)
+    const float* src = a.m0 + (long long)ul * pitch * FP;
+    float* dst = a.m2 + (long long)ul * pitch * FP;
     for (int i = tid; i < FP + 2 * nf; i += G) row[i] = 0.f;
     auto load_row = [&](int t, int slot) {
         const bool in = t >= 0 && t < T;
 #pragma unroll
         for (int j = 0; j < 4; ++j) {
             const int bin = tid + j * G;
-            ring[slot * FP + bin] = (in && bin < FF) ? src[(long long)t * FP + bin] : 0.f;
+            ring[slot * FP + bin] = (in && bin < FF) ? src[(long long)(t & rmask) * FP + bin] : 0.f;
         }
     };
     // ring slot of frame t: (t - t_begin + nt) mod R, so the newest row t + nt of step t sits at slot (t - t_begin + 2 nt) mod R
@@ -1607,7 +1621,7 @@ __global__ void __launch_bounds__(288) k_smooth_stream(const SmoothFArgs a) {
 #pragma unroll
         for (int j = 0; j < 4; ++j) {
             const int bin = tid + j * G;
-            dst[(long long)t * FP + bin] = bin < FF ? fmaf(o[j] * invD, a.p, a.one_minus_p) : 0.f;      // nonstationary.py:82-84
+            dst[(long long)(t & rmask) * FP + bin] = bin < FF ? fmaf(o[j] * invD, a.p, a.one_minus_p) : 0.f;      // nonstationary.py:82-84
         }
     }
 }
@@ -1623,7 +1637,7 @@ __global__ void __launch_bounds__(288) k_smooth_stream(const SmoothFArgs a) {
 // out[f] = sum_{g=f-nf..f} b1[g] reaches nf bins to the left); bins >= F hold zeros, and FPad - F >= 12.
 inline size_t smoothb_smem_bytes(int FPad, int nt) { return ((size_t)(2 * nt + 1) * FPad + (FPad + 32) + (FPad + 16)) * 4; }
 
-template <int NF, bool ROWS = false>
+template <int NF, bool ROWS = false, bool STREAM = false>
 __global__ void __launch_bounds__(288) k_smooth_box(const SmoothFArgs a) {
     static_assert(NF >= 1 && NF <= 12, "box smoothing handles 1 <= nf <= 12");
     B200_DYN_SMEM(float, s_buf);
@@ -1637,14 +1651,15 @@ __global__ void __launch_bounds__(288) k_smooth_box(const SmoothFArgs a) {
     const int t_begin = a.tf_lo + blockIdx.x * a.TT;
     if (t_begin >= tf_hi) return;
     const int t_end = min(t_begin + a.TT, tf_hi);
-    const float* src = a.m0 + (long long)ul * a.T * FP;
-    float* dst = a.m2 + (long long)ul * a.T * FP;
+    const int pitch = STREAM ? a.sw.ring : a.T, rmask = STREAM ? a.sw.ring - 1 : -1;    // (row t: t & rmask)
+    const float* src = a.m0 + (long long)ul * pitch * FP;
+    float* dst = a.m2 + (long long)ul * pitch * FP;
     for (int i = tid; i < 2 * FP + 48; i += G) rowA[i] = 0.f;          // rowA and rowB are contiguous
     const int b0 = 4 * tid;
     auto fetch_row = [&](int t) -> float4 {
         float4 v = make_float4(0.f, 0.f, 0.f, 0.f);
         if (t >= 0 && t < T) {
-            v = __ldg(reinterpret_cast<const float4*>(src + (long long)t * FP + b0));
+            v = __ldg(reinterpret_cast<const float4*>(src + (long long)(t & rmask) * FP + b0));
             if (b0 + 0 >= FF) v.x = 0.f;
             if (b0 + 1 >= FF) v.y = 0.f;
             if (b0 + 2 >= FF) v.z = 0.f;
@@ -1714,7 +1729,7 @@ __global__ void __launch_bounds__(288) k_smooth_box(const SmoothFArgs a) {
             r.y = b0 + 1 < FF ? fmaf(o1 * invD, a.p, a.one_minus_p) : 0.f;
             r.z = b0 + 2 < FF ? fmaf(o2 * invD, a.p, a.one_minus_p) : 0.f;
             r.w = b0 + 3 < FF ? fmaf(o3 * invD, a.p, a.one_minus_p) : 0.f;
-            *reinterpret_cast<float4*>(dst + (long long)t * FP + b0) = r;
+            *reinterpret_cast<float4*>(dst + (long long)(t & rmask) * FP + b0) = r;
         }
     }
 }
@@ -1847,34 +1862,47 @@ struct TMovArgs {
     const float* mag;
     float* m0;                 // blended sigmoid mask, prop_decrease * (m - 1) + 1 (torchgate.py:241)
     const UnitDesc* units;     // ROWS instantiations: units + (first unit of the batch); T is then the pitch only
+    StreamWin sw;              // STREAM instantiations: frames [sw.f0, f1) of the rings; T bounds the frames only
+    int f1;
+    double* run;               // STREAM: [n_units][FPad] the running sums, carried from one launch to the next
 };
 
-template <bool ROWS = false>
+// STREAM: frames [sw.f0, f1) of a stream whose rows have T frames (T = INT_MAX while the end is not known: the caller
+// then has |X| up to frame f1 + right).  The running sum is loaded from a.run, receives the same adds and subtracts in
+// the same order as the walk from t = 0 below, and is stored back, so its rounding is that of the whole-row walk.
+template <bool ROWS = false, bool STREAM = false>
 __global__ void __launch_bounds__(128) k_tgate_movmean(const TMovArgs a) {
     const long long idx = (long long)blockIdx.x * blockDim.x + threadIdx.x;
     if (idx >= (long long)a.n_units * kFPad) return;
     const int ul = (int)(idx / kFPad), f = (int)(idx - (long long)ul * kFPad);
     const int T = ROWS ? a.units[ul].T : a.T;             // ROWS: the unit's own frames (conv1d's "same" edges)
-    const float* A = a.mag + (long long)ul * a.T * kFPad + f;
-    float* M = a.m0 + (long long)ul * a.T * kFPad + f;
+    const int pitch = STREAM ? a.sw.ring : a.T, rmask = STREAM ? a.sw.ring - 1 : -1;    // (row t: t & rmask)
+    const int t0 = STREAM ? a.sw.f0 : 0, t1 = STREAM ? a.f1 : T;
+    const float* A = a.mag + (long long)ul * pitch * kFPad + f;
+    float* M = a.m0 + (long long)ul * pitch * kFPad + f;
     if (f >= kF) {
-        for (int t = 0; t < T; ++t) M[(long long)t * kFPad] = 0.f;
+        for (int t = t0; t < t1; ++t) M[(long long)(t & rmask) * kFPad] = 0.f;
         return;
     }
     // conv1d(ones(n), padding="same"): window [t - left, t + right], zero padded, left = (n-1)/2
     const int n = a.n_movemean, left = (n - 1) / 2, right = n - 1 - left;
     double run = 0.0;
-    for (int t = 0; t <= right && t < T; ++t) run += (double)A[(long long)t * kFPad];
-    for (int t = 0; t < T; ++t) {
-        const float Av = A[(long long)t * kFPad];
+    if (t0 == 0) {
+        for (int t = 0; t <= right && t < T; ++t) run += (double)A[(long long)(t & rmask) * kFPad];
+    } else {
+        run = a.run[idx];
+    }
+    for (int t = t0; t < t1; ++t) {
+        const float Av = A[(long long)(t & rmask) * kFPad];
         const float S = (float)(run / (double)n);
         const float r = (Av - S) / S;
         const float m = 1.0f / (1.0f + expf(-(r - a.n_thresh) * a.inv_temp));
-        M[(long long)t * kFPad] = a.p * (m - 1.0f) + 1.0f;
+        M[(long long)(t & rmask) * kFPad] = a.p * (m - 1.0f) + 1.0f;
         const int tin = t + 1 + right, tout = t - left;
-        if (tin < T) run += (double)A[(long long)tin * kFPad];
-        if (tout >= 0) run -= (double)A[(long long)tout * kFPad];
+        if (tin < T) run += (double)A[(long long)(tin & rmask) * kFPad];
+        if (tout >= 0) run -= (double)A[(long long)(tout & rmask) * kFPad];
     }
+    if (STREAM) a.run[idx] = run;
 }
 
 // =============================================================================================

@@ -104,7 +104,9 @@ __device__ __forceinline__ void k2c_freq_taps(const unsigned char* rows, unsigne
 #ifndef B200_K2C_MINBLOCKS
 #define B200_K2C_MINBLOCKS 3
 #endif
-template <int HR, int MK, typename T, bool ROWS = false>
+// STREAM (kMaskF32, b200gate_tstream_*): spectra and masks come from the stream's rings (K2Args::sw); the hops of a
+// launch are [pad / H + 2, ...) through Geom as usual, with y the virtual base of output sample `pad`.
+template <int HR, int MK, typename T, bool ROWS = false, bool STREAM = false>
 __global__ void __launch_bounds__(kThreads, B200_K2C_MINBLOCKS) k2c_synthesize(const K2Args a) {
     constexpr int NH = 32 / HR;             // frames overlapping one hop (win / hop)
     constexpr int MB = k2c_mask_bytes<MK>();
@@ -177,7 +179,8 @@ __global__ void __launch_bounds__(kThreads, B200_K2C_MINBLOCKS) k2c_synthesize(c
         T* yrow = ROWS ? static_cast<T*>(a.units[u].y) : static_cast<T*>(a.y) + (long long)c * g.out_stride;
         const float2* zunit = a.zcache + (long long)ul * a.zpairs * 1024;
         const unsigned short* munit = (MK == kMaskF32 || kBits) ? nullptr : a.num + (long long)ul * a.zpairs * (2 * kFPad);
-        const float* funit = (MK == kMaskF32) ? a.fmask + (long long)ul * g.T * kFPad : nullptr;
+        const float* funit = (MK == kMaskF32) ? a.fmask + (long long)ul * (STREAM ? a.sw.ring : g.T) * kFPad : nullptr;
+        const int zmask = STREAM ? (a.sw.ring >> 1) - 1 : -1, fmask_t = STREAM ? a.sw.ring - 1 : -1;
 
         float acc[32 + HR];
 #pragma unroll
@@ -191,8 +194,8 @@ __global__ void __launch_bounds__(kThreads, B200_K2C_MINBLOCKS) k2c_synthesize(c
                 const bool vb2 = tt + 1 <= t_last;
                 const unsigned mbytes = kBits ? 0u : ((MK == kMaskF32 && !vb2) ? (unsigned)(kFPad * 4) : (unsigned)MB);
                 mbar_expect_tx(bar, (unsigned)(kN * 8) + mbytes);
-                bulk_g2s_once(zbuf, zunit + (long long)(tt >> 1) * 1024, kN * 8, bar);
-                if (MK == kMaskF32) bulk_g2s(mbuf, funit + (long long)tt * kFPad, mbytes, bar);
+                bulk_g2s_once(zbuf, zunit + (long long)((tt >> 1) & zmask) * 1024, kN * 8, bar);
+                if (MK == kMaskF32) bulk_g2s(mbuf, funit + (long long)(tt & fmask_t) * kFPad, mbytes, bar);
                 else if (!kBits) bulk_g2s(mbuf, munit + (long long)(tt >> 1) * (2 * kFPad), mbytes, bar);
             }
         };

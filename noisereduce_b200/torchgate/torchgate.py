@@ -248,6 +248,149 @@ class TorchGate(torch.nn.Module):
         grad[:, :Lo] = out * env
         return grad
 
+    def stream(self, n_rows: int, _lib=None) -> "TorchGateStream":
+        """Gate live audio of n_rows rows as it arrives: the non-stationary gate, bit-identical to forward() on the whole
+        rows.  See TorchGateStream."""
+        return TorchGateStream(self, n_rows, _lib)
+
+
+class TorchGateStream:
+    """The non-stationary TorchGate on rows that arrive block by block (TorchGate.stream(n_rows)).
+
+    push(block) takes a [n_rows, n] CUDA tensor (any n >= 0) and returns the [n_rows, m] output samples that have become
+    final; finish() returns the rest.  torch.cat of everything returned, along dim 1, equals tg(x) in every bit, where x
+    is the concatenation of the blocks, however x is cut into blocks.  The rows advance together.
+
+    Every stage of the gate looks ahead a bounded distance (stft frames n_fft / 2 samples, the moving mean `right`
+    frames, the smoothing nt frames, the overlap-add one window), so after R samples per row exactly
+        samples_returned = hop * max(0, hb - 2),   hb = 2 floor(nS / 2),   nS = 2 floor(c / 2) - 1 - right - nt,
+        c = floor((R - n_fft / 2) / hop) + 1
+    have been returned (right = n - 1 - (n - 1) // 2 for n = n_movemean_nonstationary, nt the smoothing's time extent in
+    frames, 0 without smoothing; frames are analysed and synthesised in pairs).  The most samples held back is
+        latency_samples = n_fft / 2 + hop * (right + nt + 4 + e) - 1,   e = 1 if right + nt is even, else 0
+    (4863 samples, 0.304 s, at 16 kHz with the defaults).
+
+    push() enqueues on the current CUDA stream of the blocks' device and never waits for the device; keep the pushes of a
+    stream on one CUDA stream.  The stream has its own library handle, made at the first push on that block's device and
+    released by finish() (releasing it waits for the device, as destroying any handle does).  The TorchGate's attributes
+    are read once, by stream().  Covered: the non-stationary gate at n_fft = win_length = 1024, hop 256, float32 /
+    float16 / bfloat16 blocks (the output has the block's dtype), smoothing extents the lengths= form of forward()
+    runs; other settings raise NotImplementedError, before any library handle is made."""
+
+    def __init__(self, tg: "TorchGate", n_rows: int, _lib=None):
+        if not tg.nonstationary:
+            raise NotImplementedError("TorchGate.stream() needs nonstationary=True: the stationary gate's top_db floor and "
+                                      "thresholds are taken over all of a row's frames, so no sample is final before the end")
+        if not tg._tuned():
+            raise NotImplementedError("TorchGate.stream() needs the default STFT geometry (n_fft = win_length = 1024, "
+                                      f"hop_length = 256), not n_fft={tg.n_fft}, win_length={tg.win_length}, "
+                                      f"hop_length={tg.hop_length}")
+        nf, nt = tg._extents if tg.smoothing_filter is not None else (0, 0)
+        reason = _rows_smoothing_refusal(nf, nt, True)
+        if reason:
+            raise NotImplementedError(f"TorchGate.stream(): freq_mask_smooth_hz={tg.freq_mask_smooth_hz} / "
+                                      f"time_mask_smooth_ms={tg.time_mask_smooth_ms} give smoothing extents ({nf}, {nt}) "
+                                      f"bins / frames, {reason}")
+        if isinstance(n_rows, bool) or not isinstance(n_rows, (int, np.integer)) or n_rows < 1:
+            raise ValueError(f"n_rows must be a positive int, got {n_rows!r}")
+        n = int(tg.n_movemean_nonstationary)
+        if n < 1:
+            raise ValueError(f"n_movemean_nonstationary must be at least 1, got {n}")
+        self.n_rows = int(n_rows)
+        self._gate_kw = dict(nf=nf, nt=nt, params=tg._params(), window=torch.hann_window(tg.win_length).numpy())
+        self._lib = _lib
+        self._hop, self._n_fft, self._win = tg.hop_length, tg.n_fft, tg.win_length
+        self._right, self._nt = n - 1 - (n - 1) // 2, nt
+        e = 1 if (self._right + nt) % 2 == 0 else 0
+        self.latency_samples = self._n_fft // 2 + self._hop * (self._right + nt + 4 + e) - 1
+        self.samples_received = 0
+        self.samples_returned = 0
+        self._gate = None
+        self._device = self._dtype = None
+        self._finished = False
+
+    def returned_after(self, R: int) -> int:
+        """samples_returned after R samples per row (the closed form above)."""
+        if R < self._n_fft // 2:
+            return 0
+        c = (R - self._n_fft // 2) // self._hop + 1
+        nS = (c - c % 2) - 1 - self._right - self._nt
+        hb = nS - nS % 2
+        return self._hop * max(0, hb - 2)
+
+    def _open(self, block):
+        sr, _, _, n_thresh, temp, n_mm, prop, n_fft, win, hop = self._gate_kw["params"]
+        gate = _cabi.Gate(
+            lib=self._lib, surface=_cabi.SURFACE_TORCH, stationary=0, n_fft=n_fft, win_length=win, hop_length=hop,
+            n_grad_freq=self._gate_kw["nf"], n_grad_time=self._gate_kw["nt"], std_ddof=1, chunk_size=0, padding=0,
+            sr=float(sr), prop_decrease=prop, top_db=40.0, n_movemean=n_mm, thresh_n_mult=n_thresh,
+            sigmoid_slope=1.0 / temp, path_flags=0)
+        gate.set_window(self._gate_kw["window"])
+        gate.tstream_begin(self.n_rows)
+        self._gate = gate
+
+    def _ctx(self):
+        return torch.cuda.device(self._device) if self._device.type == "cuda" else _NullCtx()
+
+    def _stream(self):
+        return torch.cuda.current_stream(self._device).cuda_stream if self._device.type == "cuda" else None
+
+    @torch.no_grad()
+    def push(self, block: torch.Tensor) -> torch.Tensor:
+        """Append block ([n_rows, n] samples of every row) and return the [n_rows, m] output samples now final."""
+        if self._finished:
+            raise ValueError("TorchGateStream.push() after finish()")
+        if not isinstance(block, torch.Tensor) or block.ndim != 2 or block.shape[0] != self.n_rows:
+            shape = tuple(block.shape) if isinstance(block, torch.Tensor) else type(block).__name__
+            raise ValueError(f"a block must be a [{self.n_rows}, n] tensor, got {shape}")
+        if block.dtype == torch.float64:
+            raise NotImplementedError("TorchGateStream.push() takes float32 / float16 / bfloat16 blocks, not float64")
+        if block.dtype not in (torch.float32, torch.float16, torch.bfloat16):
+            raise ValueError(f"a block must be float32 / float16 / bfloat16, got {block.dtype}")
+        if block.requires_grad:
+            raise NotImplementedError("TorchGateStream has no backward pass: push blocks that do not require grad")
+        if self._lib is None and not block.is_cuda:
+            raise ValueError("noisereduce_b200.TorchGateStream runs on CUDA tensors only (no CPU fallback)")
+        if self._device is None:
+            self._device, self._dtype = block.device, block.dtype
+        elif block.device != self._device:
+            raise ValueError(f"every block of a stream must be on {self._device}, got {block.device}")
+        elif block.dtype != self._dtype:
+            raise ValueError(f"every block of a stream must be {self._dtype}, got {block.dtype}")
+        n = block.shape[1]
+        m = self.returned_after(self.samples_received + n) - self.samples_returned
+        with self._ctx():
+            if self._gate is None:
+                self._open(block)
+            y = torch.empty((self.n_rows, m), dtype=torch.float32, device=self._device)
+            if n > 0:
+                xf = block.detach().to(torch.float32).contiguous()
+                got = self._gate.tstream_push(xf.data_ptr(), n, xf.stride(0), y.data_ptr() if m else None, max(m, 1), m,
+                                              self._stream())
+                assert got == m, (got, m)
+        self.samples_received += n
+        self.samples_returned += m
+        return y.to(dtype=self._dtype)
+
+    @torch.no_grad()
+    def finish(self) -> torch.Tensor:
+        """The rest of the output, [n_rows, (R // hop) * hop - samples_returned]; closes the stream."""
+        if self._finished:
+            raise ValueError("TorchGateStream.finish() called twice")
+        R = self.samples_received
+        if R < 2 * self._win:
+            raise Exception(f"x must be bigger than {self._win * 2}")
+        m = (R // self._hop) * self._hop - self.samples_returned
+        with self._ctx():
+            y = torch.empty((self.n_rows, m), dtype=torch.float32, device=self._device)
+            got = self._gate.tstream_finish(y.data_ptr(), max(m, 1), m, self._stream())
+            assert got == m, (got, m)
+            self._gate.close()
+        self._gate = None
+        self._finished = True
+        self.samples_returned += m
+        return y.to(dtype=self._dtype)
+
 
 class _GateFunction(torch.autograd.Function):
     @staticmethod
