@@ -333,6 +333,28 @@ int b200gate_tstream_push(b200gate_handle* h, const float* in, int64_t n, int64_
 int b200gate_tstream_finish(b200gate_handle* h, float* out, int64_t out_stride, int64_t out_capacity, int64_t* n_out,
                             void* cuda_stream);
 
+/* ---- TorchGate.sessions(): one torch stream whose rows each hold their own session ----------------------------------
+ * The per-row form of a stream opened by b200gate_tstream_begin.  A row's session is the samples it receives between
+ * the stream's start, or the b200gate_tstream_end_rows / _reset_rows that last emptied the row, and its end; everything
+ * returned for it is bit-identical to b200gate_run on the session's samples alone, and after R samples of a session
+ * exactly 256 max(0, hb(R) - 2) of its output samples have been returned (hb as above).  A stream takes either the
+ * lockstep calls (b200gate_tstream_push / _finish) or these; the other kind returns B200GATE_ERR_STATE.
+ * b200gate_tstream_push_rows appends samples [0, n[b]) of row b of `in` (device float32 rows, stride in_stride) to row
+ * b's session for every row b, and writes the n_out[b] samples of row b that became final to out[b][0, n_out[b])
+ * (stride out_stride).  b200gate_tstream_end_rows ends the sessions of rows[0, k): the rest of row rows[i]'s output,
+ * n_out[i] samples, goes to out[i][0, n_out[i]), and the row is empty again.  Both only enqueue on cuda_stream; the row
+ * tables travel through a ring of 16 pinned slots, and a call waits only when the device is 16 slices behind (a push
+ * is one slice per 4096 samples of its longest row, an end one slice).  b200gate_tstream_reset_rows drops the sessions
+ * of rows[0, k) without output.  Errors, all before any change to the stream: B200GATE_ERR_ARG for a negative n[b],
+ * in_stride below the largest n[b], rows out of [0, n_rows) or listed twice, out_capacity below what the call returns,
+ * and an end of a row holding fewer than 2 win_length samples ("x must be bigger than 2048").  The stream's device
+ * state is fixed by b200gate_tstream_begin and released by b200gate_destroy. */
+int b200gate_tstream_push_rows(b200gate_handle* h, const float* in, const int64_t* n, int64_t in_stride, float* out,
+                               int64_t out_stride, int64_t out_capacity, int64_t* n_out, void* cuda_stream);
+int b200gate_tstream_end_rows(b200gate_handle* h, const int64_t* rows, int64_t k, float* out, int64_t out_stride,
+                              int64_t out_capacity, int64_t* n_out, void* cuda_stream);
+int b200gate_tstream_reset_rows(b200gate_handle* h, const int64_t* rows, int64_t k);
+
 int b200gate_get_stats(const b200gate_handle* h, b200gate_stats* out);
 
 /* ---- sample formats of device-resident callers ----------------------------------------------------------------------

@@ -40,6 +40,7 @@ EXPORTS = [
     "b200gate_mask_store_bytes", "b200gate_set_mask_store", "b200gate_adjoint", "b200gate_run_rows",
     "b200gate_torch_apply_masks_rows", "b200gate_noise_stats_rows", "b200gate_set_noise_threshold_rows",
     "b200gate_tstream_begin", "b200gate_tstream_push", "b200gate_tstream_finish",
+    "b200gate_tstream_push_rows", "b200gate_tstream_end_rows", "b200gate_tstream_reset_rows",
 ]
 
 
@@ -150,6 +151,15 @@ class GateLibrary:
         d.b200gate_tstream_begin.argtypes = [vp, i64]
         d.b200gate_tstream_push.argtypes = [vp, vp, i64, i64, vp, i64, i64, C.POINTER(i64), vp]
         d.b200gate_tstream_finish.argtypes = [vp, vp, i64, i64, C.POINTER(i64), vp]
+        d.b200gate_tstream_push_rows.argtypes = [vp, vp, C.POINTER(i64), i64, vp, i64, i64, C.POINTER(i64), vp]
+        d.b200gate_tstream_end_rows.argtypes = [vp, C.POINTER(i64), i64, vp, i64, i64, C.POINTER(i64), vp]
+        d.b200gate_tstream_reset_rows.argtypes = [vp, C.POINTER(i64), i64]
+
+
+def _i64p(a: np.ndarray):
+    """A C int64_t* to the data of a contiguous int64 numpy array."""
+    assert a.dtype == np.int64 and a.flags.c_contiguous
+    return a.ctypes.data_as(C.POINTER(C.c_int64))
 
 
 def format_code(dt) -> int:
@@ -421,6 +431,22 @@ class Gate:
         n_out = C.c_int64()
         self._check(self.lib.dll.b200gate_tstream_finish(self._h, out_ptr, out_stride, out_capacity, C.byref(n_out), stream))
         return n_out.value
+
+    # per-row torch streams: n and rows are int64 numpy arrays; the push / end return n_out as one
+    def tstream_push_rows(self, in_ptr, n, in_stride, out_ptr, out_stride, out_capacity, stream=None) -> np.ndarray:
+        n_out = np.empty_like(n)
+        self._check(self.lib.dll.b200gate_tstream_push_rows(self._h, in_ptr, _i64p(n), in_stride, out_ptr, out_stride,
+                                                            out_capacity, _i64p(n_out), stream))
+        return n_out
+
+    def tstream_end_rows(self, rows, out_ptr, out_stride, out_capacity, stream=None) -> np.ndarray:
+        n_out = np.empty_like(rows)
+        self._check(self.lib.dll.b200gate_tstream_end_rows(self._h, _i64p(rows), len(rows), out_ptr, out_stride,
+                                                           out_capacity, _i64p(n_out), stream))
+        return n_out
+
+    def tstream_reset_rows(self, rows):
+        self._check(self.lib.dll.b200gate_tstream_reset_rows(self._h, _i64p(rows), len(rows)))
 
     def set_range(self, mode: int, a: int = 0, b: int = 0):
         self._check(self.lib.dll.b200gate_set_range(self._h, mode, a, b))

@@ -39,6 +39,7 @@ const double kEps32 = 5.9604644775390625e-08;      // 2^-24, FP32 unit roundoff
 const double kKappa = 16.0;                        // guard band: |dX| <= kappa * eps32 * ||frame pair||_2
 thread_local std::string g_create_error;          // one handle per thread: a failed create reports through the calling thread
 const char* const kTsOpen = "a torch stream is open on this handle (b200gate_tstream_finish first)";
+constexpr int kSessSlots = 16;                     // depth of the per-row table upload ring (b200gate_tstream_push_rows)
 
 }  // namespace
 
@@ -138,6 +139,20 @@ struct b200gate_handle {
     float *d_ts_win = nullptr, *d_ts_mag = nullptr, *d_ts_m0 = nullptr, *d_ts_mask = nullptr;
     float2* d_ts_z = nullptr;
     double* d_ts_run = nullptr;
+    // TorchGate.sessions() (b200gate_tstream_push_rows / _end_rows): every row holds its own session at its own position
+    // (ts_row); each slice's per-row table (SessRow) is written into slot k of the pinned ring hp_sess and copied to slot
+    // k of d_sess on the caller's stream, and ev_sess[k] marks that copy.  A slice waits for its slot's previous copy only,
+    // so the host runs at most kSessSlots slices ahead of the device.  ts_mode: 0 until the first push, then 1 for the
+    // lockstep calls or 2 for the per-row calls; a stream takes one kind only.
+    struct TsRow { long long R = 0, lo = 0, nA = 0, nM = 0, nS = 0, ha = 2; };
+    int ts_mode = 0;
+    std::vector<TsRow> ts_row;
+    std::vector<long long> ts_y0;                  // b200gate_tstream_push_rows: each row's output offset in the call
+    SessRow* hp_sess = nullptr;
+    size_t hp_sess_bytes = 0;
+    SessRow* d_sess = nullptr;
+    std::vector<cudaEvent_t> ev_sess;
+    long long sess_slices = 0;
     // b200gate_run_rows: the call's unit table, written by the host into hp_units and copied to d_units on the call's
     // stream; ev_units marks that copy, so the next call can rewrite hp_units without waiting for the device
     UnitDesc* hp_units = nullptr;
@@ -786,10 +801,10 @@ static void launch_stationary_numerators(const b200gate_handle* h, const SmoothA
 
 // Float-mask smoothing (non-stationary gate, TorchGate moving-mean gate): the box form for 1 <= nf <= 12 (k_smooth_box,
 // compiled per nf), else the tap-loop streaming kernel, else (ring too large for shared memory) the tile kernel.
-#define B200_SMOOTH_BOX_CASE(NF_) case NF_: { auto kern_ = k_smooth_box<NF_, ROWS, STREAM>; \
+#define B200_SMOOTH_BOX_CASE(NF_) case NF_: { auto kern_ = k_smooth_box<NF_, ROWS, STREAM, SESS>; \
         if (set_attr) cudaFuncSetAttribute(kern_, cudaFuncAttributeMaxDynamicSharedMemorySize, 200 * 1024); \
         else B200_LAUNCH(kern_, grid, dim3(sa.FPad / 4), smem, st, sa); } break;
-template <bool ROWS = false, bool STREAM = false>
+template <bool ROWS = false, bool STREAM = false, bool SESS = false>
 static void smooth_box_dispatch(const SmoothFArgs& sa, int nf, dim3 grid, size_t smem, cudaStream_t st, bool set_attr) {
     switch (nf) {
         B200_SMOOTH_BOX_CASE(1) B200_SMOOTH_BOX_CASE(2) B200_SMOOTH_BOX_CASE(3) B200_SMOOTH_BOX_CASE(4)
@@ -798,20 +813,21 @@ static void smooth_box_dispatch(const SmoothFArgs& sa, int nf, dim3 grid, size_t
         default: break;
     }
 }
-// ROWS (b200gate_run_rows; sa.units set, tf_hi the largest of the batch) and STREAM (b200gate_tstream_*; sa.sw set): the
-// two streaming kernels only -- false when the ring does not fit shared memory.
-template <bool ROWS = false, bool STREAM = false>
+// ROWS (b200gate_run_rows; sa.units set, tf_hi the largest of the batch) and STREAM (b200gate_tstream_*; sa.sw set;
+// with SESS sa.rows set, tf_hi - tf_lo the largest span of a row): the two streaming kernels only -- false when the ring
+// does not fit shared memory.
+template <bool ROWS = false, bool STREAM = false, bool SESS = false>
 static bool launch_smooth_float(SmoothFArgs sa, int nf, int nt, int tf_lo, int tf_hi, int nu, int path_flags, cudaStream_t st) {
     const bool box_ok = nf >= 1 && nf <= 12 && sa.FPad - sa.F >= 12 && smoothb_smem_bytes(sa.FPad, nt) <= 200 * 1024 &&
                         !(path_flags & 32) && !(path_flags & 128);
     if (box_ok) {
         sa.TT = 256;                        // frames per strip (2 nt warm-up rows each)
         const int strips = (tf_hi - tf_lo + sa.TT - 1) / sa.TT;
-        smooth_box_dispatch<ROWS, STREAM>(sa, nf, dim3(strips, nu), smoothb_smem_bytes(sa.FPad, nt), st, false);
+        smooth_box_dispatch<ROWS, STREAM, SESS>(sa, nf, dim3(strips, nu), smoothb_smem_bytes(sa.FPad, nt), st, false);
     } else if (smooths_smem_bytes(sa.FPad, nf, nt) <= 200 * 1024 && !(path_flags & 32)) {
         sa.TT = 256;
         const int strips = (tf_hi - tf_lo + sa.TT - 1) / sa.TT;
-        auto kern_ = k_smooth_stream<ROWS, STREAM>;
+        auto kern_ = k_smooth_stream<ROWS, STREAM, SESS>;
         B200_LAUNCH(kern_, dim3(strips, nu), dim3(sa.FPad / 4), smooths_smem_bytes(sa.FPad, nf, nt), st, sa);
     } else if (ROWS || STREAM) {
         return false;
@@ -1066,6 +1082,13 @@ int b200gate_create(const b200gate_params* p, b200gate_handle** out) {
                              k2c_smem_bytes<kMaskF32>());
         cudaFuncSetAttribute(k_smooth_stream<false, true>, cudaFuncAttributeMaxDynamicSharedMemorySize, 200 * 1024);
         for (int nfb = 1; nfb <= 12; ++nfb) smooth_box_dispatch<false, true>(SmoothFArgs{}, nfb, dim3(1), 0, nullptr, true);
+        // b200gate_tstream_push_rows / _end_rows: the SESS instantiations
+        cudaFuncSetAttribute(k1n_magnitude<8, float, false, true, true>, cudaFuncAttributeMaxDynamicSharedMemorySize,
+                             k1n_smem_floats() * 4);
+        cudaFuncSetAttribute(k2c_synthesize<8, kMaskF32, float, false, true, true>, cudaFuncAttributeMaxDynamicSharedMemorySize,
+                             k2c_smem_bytes<kMaskF32>());
+        cudaFuncSetAttribute(k_smooth_stream<false, true, true>, cudaFuncAttributeMaxDynamicSharedMemorySize, 200 * 1024);
+        for (int nfb = 1; nfb <= 12; ++nfb) smooth_box_dispatch<false, true, true>(SmoothFArgs{}, nfb, dim3(1), 0, nullptr, true);
         cudaFuncSetAttribute(k2c_synthesize<8, kMaskU16, float, true>, cudaFuncAttributeMaxDynamicSharedMemorySize, k2c_smem_bytes<kMaskU16>());
         cudaFuncSetAttribute(k2c_synthesize<8, kMaskU16Blend, float, true>, cudaFuncAttributeMaxDynamicSharedMemorySize, k2c_smem_bytes<kMaskU16Blend>());
         cudaFuncSetAttribute(k1n_magnitude_2k, cudaFuncAttributeMaxDynamicSharedMemorySize, k1n2_smem_floats() * 4);
@@ -1119,6 +1142,8 @@ void b200gate_destroy(b200gate_handle* h) {
     for (int i = 0; i < 2; ++i) { g_pinned_pool.give(h->hp_in[i], h->hp_in_bytes[i]); g_pinned_pool.give(h->hp_out[i], h->hp_out_bytes[i]); }
     if (h->d_need_rowmax) cudaFree(h->d_need_rowmax);
     g_pinned_pool.give(h->hp_units, h->hp_units_bytes);
+    g_pinned_pool.give(h->hp_sess, h->hp_sess_bytes);
+    for (cudaEvent_t e : h->ev_sess) cudaEventDestroy(e);
     if (h->d_units) cudaFree(h->d_units);
     if (h->d_rtab) cudaFree(h->d_rtab);
     if (h->d_ts) cudaFree(h->d_ts);
@@ -2705,7 +2730,7 @@ int b200gate_run_rows(b200gate_handle* h, const b200gate_row* rows, int64_t n_ro
     else CK(h, cudaEventSynchronize(h->ev_units));             // the last call's table has left hp_units
     if (h->hp_units_bytes < tbytes) {
         g_pinned_pool.give(h->hp_units, h->hp_units_bytes);
-        h->hp_units = (UnitDesc*)g_pinned_pool.take(tbytes, &h->hp_units_bytes);
+        h->hp_units =(UnitDesc*)g_pinned_pool.take(tbytes, &h->hp_units_bytes);
         if (!h->hp_units) { h->hp_units_bytes = 0; return fail(h, B200GATE_ERR_NOMEM, "pinned unit table (%zu bytes)", tbytes); }
     }
     {
@@ -3466,76 +3491,100 @@ long long ts_hops_done(const b200gate_handle* h, long long R) {      // hb(R) ab
     return std::max(2LL, nS & ~1LL);
 }
 
-// Advance the stream to R = h->ts_R received samples (T = 0) or to its end (T = R / H + 1 frames): analysis, moving mean,
-// smoothing, synthesis of what has become final.  The hops returned go to out[b][0, ...) (row stride out_stride).
-int ts_advance(b200gate_handle* h, long long T, float* out, long long out_stride, cudaStream_t st) {
+// One row's stage targets after R received samples (T = 0) or at its end (T = R / H + 1 frames), from the moving mean
+// and smoothing done so far (nM0, nS0) and the first hop not yet returned (ha0): analysis to nA, moving mean to nM,
+// smoothing to nS, synthesis to hop hb.
+struct TsTarget { long long nA, nM, nS, hb; };
+TsTarget ts_target(const b200gate_handle* h, long long R, long long T, long long nM0, long long nS0, long long ha0) {
+    if (T > 0) return {T, T, T, T + 1};
+    const int n = h->p.n_movemean, right = n - 1 - (n - 1) / 2;
+    const long long c = R >= kN / 2 ? (R - kN / 2) / h->p.hop_length + 1 : 0;
+    const long long nA = c & ~1LL, nM = std::max(nM0, nA - 1 - right), nS = std::max(nS0, nM - h->p.n_grad_time);
+    return {nA, nM, nS, std::max(ha0, nS & ~1LL)};
+}
+
+// The launches of one slice: frames [a0, a1) of analysis, [m0, m1) of moving mean, [s0, s1) of smoothing and hops
+// [ha, hb) of synthesis, under the frame bound Tb (INT_MAX while the end is unknown), R samples in the window x (the
+// virtual base of sample 0), hop ha's first sample to out[b][0].  SESS: every row's ranges, bound, window start and
+// output offset come from the device table `rows`; the ranges here start at 0 and end at the largest span of any row,
+// which sizes the grids (rows with less to do leave early), and Tb, R and x are unused.
+struct TsSlice { long long a0, a1, m0, m1, s0, s1, ha, hb; int Tb; long long R; const float* x; };
+
+extern "C++" {                                             // (this file's entry points have C linkage)
+template <bool SESS>
+int ts_launch(b200gate_handle* h, const TsSlice& s, const SessRow* rows, float* out, long long out_stride, cudaStream_t st) {
     const b200gate_params& p = h->p;
     const int H = p.hop_length, nt = p.n_grad_time, nf = p.n_grad_freq, ring = h->ts_ring;
-    const int n = p.n_movemean, right = n - 1 - (n - 1) / 2;
+    const int n = p.n_movemean;
     const int B = (int)h->ts_B;
-    const bool fin = T > 0;
-    const int Tb = fin ? (int)T : INT_MAX;                   // the frame bound the kernels see
-    const long long R = h->ts_R;
-    const long long c = R >= kN / 2 ? (R - kN / 2) / H + 1 : 0;
-    const long long nA = fin ? T : (c & ~1LL);
-    const long long nM = fin ? T : std::max(h->ts_nM, nA - 1 - right);
-    const long long nS = fin ? T : std::max(h->ts_nS, nM - nt);
-    const long long hb = fin ? T + 1 : std::max(h->ts_ha, nS & ~1LL);
     const Tables tb = device_tables(h);
     StreamWin sw{};
     sw.ring = ring;
-    if (nA > h->ts_nA) {
+    if (s.a1 > s.a0) {
         K1nArgs a1{};
-        a1.g.H = H; a1.g.C = B; a1.g.T = (int)nA; a1.g.n_chunks = 1; a1.g.n_total = R; a1.g.step = R; a1.g.pad = 0;
-        a1.g.Lp = R; a1.g.in_stride = h->ts_cap; a1.g.u0 = 0; a1.g.n_units = B;
-        a1.tb = tb; a1.x = h->d_ts_win - h->ts_lo; a1.mag = h->d_ts_mag; a1.dbg.ul = -1; a1.zcache = h->d_ts_z;
+        a1.g.H = H; a1.g.C = B; a1.g.T = (int)s.a1; a1.g.n_chunks = 1; a1.g.n_total = s.R; a1.g.step = s.R; a1.g.pad = 0;
+        a1.g.Lp = s.R; a1.g.in_stride = h->ts_cap; a1.g.u0 = 0; a1.g.n_units = B;
+        a1.tb = tb; a1.x = SESS ? h->d_ts_win : s.x; a1.mag = h->d_ts_mag; a1.dbg.ul = -1; a1.zcache = h->d_ts_z;
         a1.zpairs = ring / 2; a1.z_lo = 0; a1.z_hi = INT_MAX;
-        sw.f0 = (int)h->ts_nA;
-        a1.sw = sw;
+        sw.f0 = (int)s.a0;
+        a1.sw = sw; a1.rows = rows;
         a1.run = 2;                                           // one frame pair per work item (pairs are global either way)
-        a1.n_runs = (int)((nA - h->ts_nA + 1) / 2);
-        auto kern_ = k1n_magnitude<8, float, false, true>;
+        a1.n_runs = (int)((s.a1 - s.a0 + 1) / 2);
+        auto kern_ = k1n_magnitude<8, float, false, true, SESS>;
         B200_LAUNCH(kern_, dim3(grid_1d((long long)B * a1.n_runs, kWarps, h->num_sm * 3)), dim3(kThreads),
                     k1n_smem_floats() * 4, st, a1);
     }
-    if (nM > h->ts_nM) {
+    if (s.m1 > s.m0) {
         TMovArgs ma{};
-        ma.n_units = B; ma.T = Tb; ma.n_movemean = n; ma.n_thresh = (float)p.thresh_n_mult;
+        ma.n_units = B; ma.T = s.Tb; ma.n_movemean = n; ma.n_thresh = (float)p.thresh_n_mult;
         ma.inv_temp = (float)p.sigmoid_slope; ma.p = (float)p.prop_decrease; ma.mag = h->d_ts_mag; ma.m0 = h->d_ts_m0;
-        sw.f0 = (int)h->ts_nM;
-        ma.sw = sw; ma.f1 = (int)nM; ma.run = h->d_ts_run;
-        auto kern_ = k_tgate_movmean<false, true>;
+        sw.f0 = (int)s.m0;
+        ma.sw = sw; ma.f1 = (int)s.m1; ma.run = h->d_ts_run; ma.rows = rows;
+        auto kern_ = k_tgate_movmean<false, true, SESS>;
         B200_LAUNCH(kern_, dim3(grid_1d((long long)B * kFPad, 128, 1 << 30)), dim3(128), 0, st, ma);
     }
-    if (nS > h->ts_nS) {
+    if (s.s1 > s.s0) {
         SmoothFArgs sa{};
-        sa.n_units = B; sa.T = Tb; sa.nf = nf; sa.nt = nt; sa.tf_lo = (int)h->ts_nS; sa.tf_hi = (int)nS; sa.F = kF; sa.FPad = kFPad;
+        sa.n_units = B; sa.T = s.Tb; sa.nf = nf; sa.nt = nt; sa.tf_lo = (int)s.s0; sa.tf_hi = (int)s.s1; sa.F = kF; sa.FPad = kFPad;
         sa.p = 1.0f; sa.one_minus_p = 0.0f;                  // (the torch surface blends in k_tgate_movmean)
-        sa.m0 = h->d_ts_m0; sa.m2 = h->d_ts_mask; sa.sw = sw;
-        launch_smooth_float<false, true>(sa, nf, nt, (int)h->ts_nS, (int)nS, B, 0, st);   // (extents checked at begin)
+        sa.m0 = h->d_ts_m0; sa.m2 = h->d_ts_mask; sa.sw = sw; sa.rows = rows;
+        launch_smooth_float<false, true, SESS>(sa, nf, nt, (int)s.s0, (int)s.s1, B, 0, st);   // (extents checked at begin)
     }
-    if (hb > h->ts_ha) {
+    if (s.hb > s.ha) {
         // hops [ha, hb): Geom's padded-chunk view with pad = (ha - 2) H puts the first of them at h_lo and output sample
         // (ha - 2) H at out[b][0]; while the end is unknown, T = hb + 1 keeps every hop interior
-        const long long P = (h->ts_ha - 2) * H;
-        const long long out_len = (fin ? (T - 1) * H : (hb - 2) * H) - P;
+        const long long P = (s.ha - 2) * H;
+        const long long out_len = (s.hb - 2) * H - P;
         K2Args a2{};
-        a2.g.H = H; a2.g.C = B; a2.g.T = fin ? (int)T : (int)hb + 1; a2.g.n_chunks = 1; a2.g.n_total = out_len;
+        a2.g.H = H; a2.g.C = B; a2.g.T = (int)std::min<long long>(s.Tb, s.hb + 1); a2.g.n_chunks = 1; a2.g.n_total = out_len;
         a2.g.step = out_len; a2.g.pad = P; a2.g.Lp = out_len + P; a2.g.out_stride = out_stride; a2.g.u0 = 0; a2.g.n_units = B;
         a2.tb = tb; a2.y = out; a2.fmask = h->d_ts_mask; a2.zcache = h->d_ts_z; a2.zpairs = ring / 2; a2.nt = nt;
-        a2.dbg.ul = -1; a2.sw = sw;
-        const long long hops = hb - h->ts_ha;
+        a2.dbg.ul = -1; a2.sw = sw; a2.rows = rows;
+        const long long hops = s.hb - s.ha;
         long long want = (long long)h->num_sm * 3 * kWarps * 4;
         long long run = std::max(16LL, std::min(128LL, ((long long)B * hops + want - 1) / want));
         run += run & 1;                                       // work items end on odd frames, as in b200gate_run
         a2.run = (int)run;
         a2.n_runs = (int)((hops + run - 1) / run);
-        auto kern_ = k2c_synthesize<8, kMaskF32, float, false, true>;
+        auto kern_ = k2c_synthesize<8, kMaskF32, float, false, true, SESS>;
         B200_LAUNCH(kern_, dim3(grid_1d((long long)B * a2.n_runs, kWarps, h->num_sm * 3)), dim3(kThreads),
                     k2c_smem_bytes<kMaskF32>(), st, a2);
     }
     CK(h, cudaGetLastError());
-    h->ts_nA = nA; h->ts_nM = nM; h->ts_nS = nS; h->ts_ha = hb;
+    return B200GATE_OK;
+}
+}  // extern "C++"
+
+// Advance the lockstep stream to R = h->ts_R received samples (T = 0) or to its end (T = R / H + 1 frames): analysis,
+// moving mean, smoothing, synthesis of what has become final.  The hops returned go to out[b][0, ...) (row stride
+// out_stride).
+int ts_advance(b200gate_handle* h, long long T, float* out, long long out_stride, cudaStream_t st) {
+    const TsTarget t = ts_target(h, h->ts_R, T, h->ts_nM, h->ts_nS, h->ts_ha);
+    const TsSlice s{h->ts_nA, t.nA, h->ts_nM, t.nM, h->ts_nS, t.nS, h->ts_ha, t.hb, T > 0 ? (int)T : INT_MAX, h->ts_R,
+                    h->d_ts_win - h->ts_lo};
+    const int rc = ts_launch<false>(h, s, nullptr, out, out_stride, st);
+    if (rc) return rc;
+    h->ts_nA = t.nA; h->ts_nM = t.nM; h->ts_nS = t.nS; h->ts_ha = t.hb;
     return B200GATE_OK;
 }
 
@@ -3543,6 +3592,67 @@ void ts_release(b200gate_handle* h) {
     if (h->d_ts) cudaFree(h->d_ts);
     h->d_ts = nullptr;
     h->ts_open = false;
+    h->ts_mode = 0;
+}
+
+const char* const kTsLockstep = "this torch stream advances its rows together (b200gate_tstream_push / _finish)";
+const char* const kTsPerRow = "this torch stream advances its rows one by one (b200gate_tstream_push_rows / _end_rows / _reset_rows)";
+
+// The per-row calls: an open stream that has not taken the lockstep calls.
+int sess_check(b200gate_handle* h) {
+    if (!h->ts_open) return fail(h, B200GATE_ERR_STATE, "no open torch stream (b200gate_tstream_begin first)");
+    if (h->ts_mode == 1) return fail(h, B200GATE_ERR_STATE, kTsLockstep);
+    return B200GATE_OK;
+}
+
+// rows[0, k): in range and none twice
+int sess_check_rows(b200gate_handle* h, const int64_t* rows, int64_t k) {
+    if (k < 0 || (k > 0 && !rows)) return fail(h, B200GATE_ERR_ARG, "bad argument");
+    std::vector<char> seen((size_t)h->ts_B, 0);
+    for (int64_t i = 0; i < k; ++i) {
+        if (rows[i] < 0 || rows[i] >= h->ts_B)
+            return fail(h, B200GATE_ERR_ARG, "row %lld out of range [0, %lld)", (long long)rows[i], h->ts_B);
+        if (seen[(size_t)rows[i]]++) return fail(h, B200GATE_ERR_ARG, "row %lld listed twice", (long long)rows[i]);
+    }
+    return B200GATE_OK;
+}
+
+// Row r's table entry for a slice that brings it to r.R samples (T = 0) or ends it (T = R / H + 1); its output sample j
+// goes to out[y + j].  Advances r and widens the largest spans in `span`.
+void sess_fill(const b200gate_handle* h, b200gate_handle::TsRow& r, SessRow& e, long long T, long long y, TsSlice& span) {
+    const TsTarget t = ts_target(h, r.R, T, r.nM, r.nS, r.ha);
+    e.R = r.R; e.lo = r.lo; e.y = y; e.T = T > 0 ? (int)T : INT_MAX;
+    e.a0 = (int)r.nA; e.a1 = (int)t.nA; e.m0 = (int)r.nM; e.m1 = (int)t.nM;
+    e.s0 = (int)r.nS; e.s1 = (int)t.nS; e.ha = (int)r.ha; e.hb = (int)t.hb;
+    span.a1 = std::max(span.a1, t.nA - r.nA); span.m1 = std::max(span.m1, t.nM - r.nM);
+    span.s1 = std::max(span.s1, t.nS - r.nS); span.hb = std::max(span.hb, t.hb - r.ha);
+    r.nA = t.nA; r.nM = t.nM; r.nS = t.nS; r.ha = t.hb;
+}
+
+// The next slot of the upload ring; waits for that slot's previous copy to have left it (the only wait of the per-row
+// calls: it happens when the host is kSessSlots slices ahead of the device).
+SessRow* sess_slot(b200gate_handle* h, int* k) {
+    *k = (int)(h->sess_slices++ % kSessSlots);
+    cudaEventSynchronize(h->ev_sess[*k]);
+    SessRow* tab = h->hp_sess + (size_t)*k * h->ts_B;
+    memset(tab, 0, (size_t)h->ts_B * sizeof(SessRow));
+    for (long long b = 0; b < h->ts_B; ++b) { tab[b].ha = tab[b].hb = 2; tab[b].T = INT_MAX; }   // (nothing to do)
+    return tab;
+}
+
+// Upload slot k's table and enqueue its slice: the copy-in of block columns [off, off + S) (in != nullptr), then the
+// four stages.
+int sess_submit(b200gate_handle* h, int k, const TsSlice& span, const float* in, long long in_stride, long long off,
+                float* out, cudaStream_t st) {
+    const long long B = h->ts_B;
+    SessRow* d_tab = h->d_sess + (size_t)k * B;
+    CK(h, cudaMemcpyAsync(d_tab, h->hp_sess + (size_t)k * B, (size_t)B * sizeof(SessRow), cudaMemcpyHostToDevice, st));
+    CK(h, cudaEventRecord(h->ev_sess[k], st));
+    if (in) {
+        SessCopyArgs ca{in, in_stride, off, h->d_ts_win, h->ts_cap, d_tab};
+        B200_LAUNCH(k_sess_copy_in, dim3((unsigned)B), dim3(256), 0, st, ca);
+    }
+    return ts_launch<true>(h, span, d_tab, out, 0, st);
 }
 
 }  // namespace
@@ -3578,7 +3688,17 @@ int b200gate_tstream_begin(b200gate_handle* h, int64_t n_rows) {
     auto al = [](size_t v) { return (v + 255) / 256 * 256; };
     const size_t o_win = 0, o_z = o_win + al(B * cap * 4), o_mag = o_z + al(B * (size_t)(ring / 2) * 1024 * 8);
     const size_t o_m0 = o_mag + al(B * ring * kFPad * 4), o_mask = o_m0 + al(B * ring * kFPad * 4);
-    const size_t o_run = o_mask + al(B * ring * kFPad * 4), bytes = o_run + al(B * kFPad * 8);
+    const size_t o_run = o_mask + al(B * ring * kFPad * 4), o_sess = o_run + al(B * kFPad * 8);
+    const size_t sess_bytes = (size_t)kSessSlots * B * sizeof(SessRow), bytes = o_sess + al(sess_bytes);
+    if (h->ev_sess.empty()) {
+        h->ev_sess.assign(kSessSlots, nullptr);
+        for (cudaEvent_t& ev : h->ev_sess) CK(h, cudaEventCreateWithFlags(&ev, cudaEventDisableTiming));
+    }
+    if (h->hp_sess_bytes < sess_bytes) {
+        g_pinned_pool.give(h->hp_sess, h->hp_sess_bytes);
+        h->hp_sess = (SessRow*)g_pinned_pool.take(sess_bytes, &h->hp_sess_bytes);
+        if (!h->hp_sess) { h->hp_sess_bytes = 0; return fail(h, B200GATE_ERR_NOMEM, "pinned row tables (%zu bytes)", sess_bytes); }
+    }
     cudaError_t e = cudaMalloc(&h->d_ts, bytes);
     if (e != cudaSuccess) {
         cudaGetLastError();
@@ -3588,6 +3708,9 @@ int b200gate_tstream_begin(b200gate_handle* h, int64_t n_rows) {
     char* base = (char*)h->d_ts;
     h->d_ts_win = (float*)(base + o_win); h->d_ts_z = (float2*)(base + o_z); h->d_ts_mag = (float*)(base + o_mag);
     h->d_ts_m0 = (float*)(base + o_m0); h->d_ts_mask = (float*)(base + o_mask); h->d_ts_run = (double*)(base + o_run);
+    h->d_sess = (SessRow*)(base + o_sess);
+    h->ts_row.assign(B, b200gate_handle::TsRow{});
+    h->ts_y0.assign(B, 0);
     h->ts_B = n_rows; h->ts_R = 0; h->ts_lo = 0; h->ts_cap = cap; h->ts_slice = S; h->ts_ring = (int)ring;
     h->ts_nA = 0; h->ts_nM = 0; h->ts_nS = 0; h->ts_ha = 2;
     h->ts_open = true;
@@ -3601,11 +3724,13 @@ int b200gate_tstream_push(b200gate_handle* h, const float* in, int64_t n, int64_
     if (!n_out || n < 0 || (n > 0 && (!in || in_stride < n)) || out_capacity < 0 || (out_capacity > 0 && !out) ||
         (h->ts_B > 1 && out_stride < out_capacity))
         return fail(h, B200GATE_ERR_ARG, "bad argument");
+    if (h->ts_mode == 2) return fail(h, B200GATE_ERR_STATE, kTsPerRow);
     const long long H = h->p.hop_length;
     const long long m = (ts_hops_done(h, h->ts_R + n) - h->ts_ha) * H;
     if (out_capacity < m)
         return fail(h, B200GATE_ERR_ARG, "out_capacity %lld < %lld samples returned by this push", (long long)out_capacity, m);
     *n_out = m;
+    h->ts_mode = 1;
     if (n == 0) return B200GATE_OK;
     cudaStream_t st = (cudaStream_t)stream;
     const long long B = h->ts_B, S = h->ts_slice, ha0 = h->ts_ha;
@@ -3637,6 +3762,7 @@ int b200gate_tstream_finish(b200gate_handle* h, float* out, int64_t out_stride, 
     if (!h->ts_open) return fail(h, B200GATE_ERR_STATE, "no open torch stream (b200gate_tstream_begin first)");
     if (!n_out || out_capacity < 0 || (out_capacity > 0 && !out) || (h->ts_B > 1 && out_stride < out_capacity))
         return fail(h, B200GATE_ERR_ARG, "bad argument");
+    if (h->ts_mode == 2) return fail(h, B200GATE_ERR_STATE, kTsPerRow);
     const long long H = h->p.hop_length, R = h->ts_R;
     if (R < 2 * h->p.win_length) return fail(h, B200GATE_ERR_ARG, "x must be bigger than %d", 2 * h->p.win_length);
     const long long T = R / H + 1, m = (T + 1 - h->ts_ha) * H;      // the rest of torch.istft's (T - 1) H samples
@@ -3646,6 +3772,101 @@ int b200gate_tstream_finish(b200gate_handle* h, float* out, int64_t out_stride, 
     const int rc = ts_advance(h, T, out, out_stride, (cudaStream_t)stream);
     ts_release(h);                                            // (cudaFree waits for the device)
     return rc;
+}
+
+int b200gate_tstream_push_rows(b200gate_handle* h, const float* in, const int64_t* n, int64_t in_stride, float* out,
+                               int64_t out_stride, int64_t out_capacity, int64_t* n_out, void* stream) {
+    if (!h) return B200GATE_ERR_ARG;
+    int rc;
+    if ((rc = sess_check(h))) return rc;
+    const long long B = h->ts_B, H = h->p.hop_length, S = h->ts_slice;
+    if (!n || !n_out || out_capacity < 0 || (out_capacity > 0 && !out) || (B > 1 && out_stride < out_capacity))
+        return fail(h, B200GATE_ERR_ARG, "bad argument");
+    long long n_max = 0, m_max = 0;
+    for (long long b = 0; b < B; ++b) {
+        if (n[b] < 0) return fail(h, B200GATE_ERR_ARG, "row %lld: a negative sample count (%lld)", b, (long long)n[b]);
+        n_max = std::max(n_max, (long long)n[b]);
+        m_max = std::max(m_max, (ts_hops_done(h, h->ts_row[b].R + n[b]) - h->ts_row[b].ha) * H);
+    }
+    if (n_max > 0 && (!in || (B > 1 && in_stride < n_max))) return fail(h, B200GATE_ERR_ARG, "bad argument");
+    if (out_capacity < m_max)
+        return fail(h, B200GATE_ERR_ARG, "out_capacity %lld < %lld samples returned by this push", (long long)out_capacity, m_max);
+    for (long long b = 0; b < B; ++b) n_out[b] = (ts_hops_done(h, h->ts_row[b].R + n[b]) - h->ts_row[b].ha) * H;
+    h->ts_mode = 2;
+    cudaStream_t st = (cudaStream_t)stream;
+    std::vector<long long>& y0 = h->ts_y0;               // row b's output sample j goes to out[y0[b] + j] in this call
+    for (long long b = 0; b < B; ++b) y0[b] = b * out_stride - (h->ts_row[b].ha - 2) * H;
+    for (long long off = 0; off < n_max; off += S) {
+        int k;
+        SessRow* tab = sess_slot(h, &k);
+        TsSlice span{};
+        span.Tb = INT_MAX;
+        for (long long b = 0; b < B; ++b) {
+            b200gate_handle::TsRow& r = h->ts_row[b];
+            const long long s = std::max(0LL, std::min(S, (long long)n[b] - off));
+            if (s == 0) continue;
+            SessRow& e = tab[b];
+            e.n = (int)s;
+            e.keep = r.R - r.lo;
+            if (r.R - r.lo + s > h->ts_cap) {               // compact: keep the samples of frames nA on
+                const long long lo = std::max(0LL, r.nA * H - kN / 2);
+                e.keep = r.R - lo;
+                e.shift = lo - r.lo;
+                r.lo = lo;
+            }
+            r.R += s;
+            sess_fill(h, r, e, 0, y0[b], span);
+        }
+        if ((rc = sess_submit(h, k, span, in, in_stride, off, out, st))) {
+            ts_release(h);
+            return rc;
+        }
+    }
+    return B200GATE_OK;
+}
+
+int b200gate_tstream_end_rows(b200gate_handle* h, const int64_t* rows, int64_t k, float* out, int64_t out_stride,
+                              int64_t out_capacity, int64_t* n_out, void* stream) {
+    if (!h) return B200GATE_ERR_ARG;
+    int rc;
+    if ((rc = sess_check(h))) return rc;
+    if ((k > 0 && !n_out) || out_capacity < 0 || (out_capacity > 0 && !out) || (k > 1 && out_stride < out_capacity))
+        return fail(h, B200GATE_ERR_ARG, "bad argument");
+    if ((rc = sess_check_rows(h, rows, k))) return rc;
+    const long long H = h->p.hop_length;
+    long long m_max = 0;
+    for (int64_t i = 0; i < k; ++i) {
+        const b200gate_handle::TsRow& r = h->ts_row[rows[i]];
+        if (r.R < 2 * h->p.win_length)
+            return fail(h, B200GATE_ERR_ARG, "x must be bigger than %d (row %lld holds %lld samples)", 2 * h->p.win_length,
+                        (long long)rows[i], r.R);
+        m_max = std::max(m_max, (r.R / H + 2 - r.ha) * H);     // the rest of torch.istft's (R / H) H samples
+    }
+    if (out_capacity < m_max)
+        return fail(h, B200GATE_ERR_ARG, "out_capacity %lld < %lld samples returned by end", (long long)out_capacity, m_max);
+    if (k == 0) return B200GATE_OK;
+    h->ts_mode = 2;
+    int slot;
+    SessRow* tab = sess_slot(h, &slot);
+    TsSlice span{};
+    span.Tb = INT_MAX;
+    for (int64_t i = 0; i < k; ++i) {
+        b200gate_handle::TsRow& r = h->ts_row[rows[i]];
+        n_out[i] = (r.R / H + 2 - r.ha) * H;
+        sess_fill(h, r, tab[rows[i]], r.R / H + 1, i * out_stride - (r.ha - 2) * H, span);
+        r = b200gate_handle::TsRow{};                         // the row's next samples start a new session
+    }
+    if ((rc = sess_submit(h, slot, span, nullptr, 0, 0, out, (cudaStream_t)stream))) ts_release(h);
+    return rc;
+}
+
+int b200gate_tstream_reset_rows(b200gate_handle* h, const int64_t* rows, int64_t k) {
+    if (!h) return B200GATE_ERR_ARG;
+    int rc;
+    if ((rc = sess_check(h)) || (rc = sess_check_rows(h, rows, k))) return rc;
+    h->ts_mode = 2;
+    for (int64_t i = 0; i < k; ++i) h->ts_row[rows[i]] = b200gate_handle::TsRow{};
+    return B200GATE_OK;
 }
 
 

@@ -78,6 +78,45 @@ struct StreamWin {
     int ring;
 };
 
+// TorchGate.sessions() (b200gate_tstream_push_rows / _end_rows): every row of a stream holds its own session, so the
+// kernels templated with SESS (always with STREAM) read the row's window and frame ranges from this table, one entry per
+// row, rewritten for every slice of a push.  An empty range is a row with nothing to do in that stage.
+struct SessRow {
+    long long R;            // samples of the row's session, this slice's included
+    long long lo;           // the window holds samples [lo, R): sample j at win[row][j - lo]
+    long long y;            // output sample j of the session goes to y[this + j] (K2Args::y)
+    long long keep, shift;  // k_sess_copy_in: keep samples move from win[row][shift] to win[row][0] (shift > 0 only);
+                            // then n samples of in[row][off, off + n) are appended at win[row][keep]
+    int n;
+    int a0, a1;             // analysis frames [a0, a1), a0 even
+    int m0, m1;             // moving-mean frames
+    int s0, s1;             // smoothing frames
+    int ha, hb;             // synthesis hops [ha, hb), ha even
+    int T;                  // the frame bound: INT_MAX while the session is live, R / H + 1 in the end() that finishes it
+};
+
+struct SessCopyArgs {
+    const float* in;        // [rows][in_stride]; this slice starts at column off
+    long long in_stride, off;
+    float* win;             // [rows][cap]
+    long long cap;
+    const SessRow* rows;
+};
+
+// One CTA per row.  keep < 2 H + n_fft <= shift (the window pitch leaves that much room behind the kept span), so the
+// move reads and writes disjoint spans; the append, which may overwrite the span moved from, follows a barrier.
+__global__ void __launch_bounds__(256) k_sess_copy_in(const SessCopyArgs a) {
+    const int b = blockIdx.x;
+    const SessRow& r = a.rows[b];
+    if (r.n == 0) return;
+    float* w = a.win + (long long)b * a.cap;
+    if (r.shift > 0)
+        for (long long i = threadIdx.x; i < r.keep; i += blockDim.x) w[i] = w[r.shift + i];
+    __syncthreads();
+    const float* src = a.in + (long long)b * a.in_stride + a.off;
+    for (long long i = threadIdx.x; i < r.n; i += blockDim.x) w[r.keep + i] = __ldg(src + i);
+}
+
 struct Tables {              // device pointers, built once per handle
     const float* wa;         // [N] analysis window / sum(w)
     const float* ws;         // [N] synthesis window * sum(w) / N
@@ -949,6 +988,7 @@ struct K2Args {
     long long adj_pitch;
     const UnitDesc* units;         // k2c_synthesize<.., ROWS = true>: the call's unit table
     StreamWin sw;                  // k2c_synthesize<.., STREAM = true>: zcache / fmask are the stream's rings (zpairs = ring / 2)
+    const SessRow* rows;           // k2c_synthesize<.., SESS = true>: row ul's hops [ha, hb), bound T and output offset
 };
 
 constexpr int k2_smem_floats(int H) { return 2 * kN + 2 * kN + H + kFPad + kWarps * kExchFloats + 8 + kWarps * 2 * kN; }
@@ -1280,11 +1320,12 @@ struct K1nArgs {
     int z_lo, z_hi;
     const UnitDesc* units;     // ROWS instantiations: the call's unit table
     StreamWin sw;              // STREAM instantiations: frames [sw.f0, g.T) into the rings
+    const SessRow* rows;       // SESS instantiations: row ul's window and frames [a0, a1); x is the window, g.in_stride its pitch
 };
 
 constexpr int k1n_smem_floats() { return kN + 2 * kN + kWarps * kExchFloats; }
 
-template <int HR, typename T, bool ROWS = false, bool STREAM = false>
+template <int HR, typename T, bool ROWS = false, bool STREAM = false, bool SESS = false>
 __global__ void __launch_bounds__(kThreads, 3) k1n_magnitude(const K1nArgs a) {
     B200_DYN_SMEM(float, smem);
     float* s_wa = smem;
@@ -1308,11 +1349,13 @@ __global__ void __launch_bounds__(kThreads, 3) k1n_magnitude(const K1nArgs a) {
         const int u = g.u0 + ul;
         const int ic = u / g.C, c = u - ic * g.C;
         const UnitDesc* d = ROWS ? a.units + u : nullptr;        // ROWS: the unit's own row, span and frames
+        const SessRow* sr = SESS ? a.rows + ul : nullptr;        // SESS: the row's own window and frames
         const long long i1 = ROWS ? d->i1 : (long long)ic * g.step - g.pad;
-        const T* xrow = ROWS ? static_cast<const T*>(d->x) : static_cast<const T*>(a.x) + (long long)c * g.in_stride;
-        const long long Lp_u = ROWS ? d->Lp : g.Lp, n_u = ROWS ? d->n_total : g.n_total;
-        const int T_u = ROWS ? d->T : g.T;
-        const int t0 = (STREAM ? a.sw.f0 : 0) + run * a.run;
+        const T* xrow = ROWS ? static_cast<const T*>(d->x)
+                             : static_cast<const T*>(a.x) + (long long)c * g.in_stride - (SESS ? sr->lo : 0);
+        const long long Lp_u = ROWS ? d->Lp : SESS ? sr->R : g.Lp, n_u = ROWS ? d->n_total : SESS ? sr->R : g.n_total;
+        const int T_u = ROWS ? d->T : SESS ? sr->a1 : g.T;
+        const int t0 = (SESS ? sr->a0 : STREAM ? a.sw.f0 : 0) + run * a.run;
         const int t1 = min(t0 + a.run, T_u);
         for (int t = t0; t < t1; t += 2) {
             const bool vb = (t + 1 < t1);
@@ -1518,6 +1561,7 @@ struct SmoothFArgs {
     const UnitDesc* units;     // ROWS instantiations: units + (first unit of the batch); T is then the pitch only and
                                // tf_hi the largest of the batch
     StreamWin sw;              // STREAM instantiations: m0 / m2 are rings of sw.ring rows; T bounds the frames only
+    const SessRow* rows;       // SESS instantiations: row ul's frames [s0, s1) and bound T (tf_lo, tf_hi and T unused)
 };
 __host__ __device__ inline int smoothf_cpitch(int FPad, int nf) { return FPad + 2 * nf + 1; }
 inline size_t smoothf_smem_bytes(int TT, int FPad, int nf) { return (size_t)TT * smoothf_cpitch(FPad, nf) * 4; }
@@ -1568,7 +1612,7 @@ __global__ void __launch_bounds__(256) k_smooth_f(const SmoothFArgs a) {
 // once per strip and written once.
 inline size_t smooths_smem_bytes(int FPad, int nf, int nt) { return ((size_t)(2 * nt + 1) * FPad + FPad + 2 * nf + 8) * 4; }
 
-template <bool ROWS = false, bool STREAM = false>
+template <bool ROWS = false, bool STREAM = false, bool SESS = false>
 __global__ void __launch_bounds__(288) k_smooth_stream(const SmoothFArgs a) {
     B200_DYN_SMEM(float, s_buf);
     const int FP = a.FPad, FF = a.F, nt = a.nt, nf = a.nf, R = 2 * nt + 1;
@@ -1576,8 +1620,9 @@ __global__ void __launch_bounds__(288) k_smooth_stream(const SmoothFArgs a) {
     float* ring = s_buf;                     // [R][FP]
     float* row = s_buf + (size_t)R * FP;     // [nf | FP | nf]
     const int ul = blockIdx.y;
-    const int T = ROWS ? a.units[ul].T : a.T, tf_hi = ROWS ? a.units[ul].tf_hi : a.tf_hi;
-    const int t_begin = a.tf_lo + blockIdx.x * a.TT;
+    const int T = ROWS ? a.units[ul].T : SESS ? a.rows[ul].T : a.T;
+    const int tf_hi = ROWS ? a.units[ul].tf_hi : SESS ? a.rows[ul].s1 : a.tf_hi;
+    const int t_begin = (SESS ? a.rows[ul].s0 : a.tf_lo) + blockIdx.x * a.TT;
     if (t_begin >= tf_hi) return;
     const int t_end = min(t_begin + a.TT, tf_hi);
     const int pitch = STREAM ? a.sw.ring : a.T, rmask = STREAM ? a.sw.ring - 1 : -1;    // (row t: t & rmask)
@@ -1637,7 +1682,7 @@ __global__ void __launch_bounds__(288) k_smooth_stream(const SmoothFArgs a) {
 // out[f] = sum_{g=f-nf..f} b1[g] reaches nf bins to the left); bins >= F hold zeros, and FPad - F >= 12.
 inline size_t smoothb_smem_bytes(int FPad, int nt) { return ((size_t)(2 * nt + 1) * FPad + (FPad + 32) + (FPad + 16)) * 4; }
 
-template <int NF, bool ROWS = false, bool STREAM = false>
+template <int NF, bool ROWS = false, bool STREAM = false, bool SESS = false>
 __global__ void __launch_bounds__(288) k_smooth_box(const SmoothFArgs a) {
     static_assert(NF >= 1 && NF <= 12, "box smoothing handles 1 <= nf <= 12");
     B200_DYN_SMEM(float, s_buf);
@@ -1647,8 +1692,9 @@ __global__ void __launch_bounds__(288) k_smooth_box(const SmoothFArgs a) {
     float* rowA = s_buf + (size_t)R * FP;                  // [16 | FP | 16]
     float* rowB = rowA + FP + 32;                          // [FP + 16]
     const int ul = blockIdx.y;
-    const int T = ROWS ? a.units[ul].T : a.T, tf_hi = ROWS ? a.units[ul].tf_hi : a.tf_hi;
-    const int t_begin = a.tf_lo + blockIdx.x * a.TT;
+    const int T = ROWS ? a.units[ul].T : SESS ? a.rows[ul].T : a.T;
+    const int tf_hi = ROWS ? a.units[ul].tf_hi : SESS ? a.rows[ul].s1 : a.tf_hi;
+    const int t_begin = (SESS ? a.rows[ul].s0 : a.tf_lo) + blockIdx.x * a.TT;
     if (t_begin >= tf_hi) return;
     const int t_end = min(t_begin + a.TT, tf_hi);
     const int pitch = STREAM ? a.sw.ring : a.T, rmask = STREAM ? a.sw.ring - 1 : -1;    // (row t: t & rmask)
@@ -1865,19 +1911,23 @@ struct TMovArgs {
     StreamWin sw;              // STREAM instantiations: frames [sw.f0, f1) of the rings; T bounds the frames only
     int f1;
     double* run;               // STREAM: [n_units][FPad] the running sums, carried from one launch to the next
+    const SessRow* rows;       // SESS instantiations: row ul's frames [m0, m1) and bound T (sw.f0, f1 and T unused)
 };
 
 // STREAM: frames [sw.f0, f1) of a stream whose rows have T frames (T = INT_MAX while the end is not known: the caller
 // then has |X| up to frame f1 + right).  The running sum is loaded from a.run, receives the same adds and subtracts in
 // the same order as the walk from t = 0 below, and is stored back, so its rounding is that of the whole-row walk.
-template <bool ROWS = false, bool STREAM = false>
+// SESS: the same per row; a session's first launch starts at frame 0 and builds the sum afresh, so a row that starts a
+// new session never reads the sum its previous session left.
+template <bool ROWS = false, bool STREAM = false, bool SESS = false>
 __global__ void __launch_bounds__(128) k_tgate_movmean(const TMovArgs a) {
     const long long idx = (long long)blockIdx.x * blockDim.x + threadIdx.x;
     if (idx >= (long long)a.n_units * kFPad) return;
     const int ul = (int)(idx / kFPad), f = (int)(idx - (long long)ul * kFPad);
-    const int T = ROWS ? a.units[ul].T : a.T;             // ROWS: the unit's own frames (conv1d's "same" edges)
+    const int T = ROWS ? a.units[ul].T : SESS ? a.rows[ul].T : a.T;   // ROWS: the unit's own frames (conv1d's "same" edges)
     const int pitch = STREAM ? a.sw.ring : a.T, rmask = STREAM ? a.sw.ring - 1 : -1;    // (row t: t & rmask)
-    const int t0 = STREAM ? a.sw.f0 : 0, t1 = STREAM ? a.f1 : T;
+    const int t0 = SESS ? a.rows[ul].m0 : STREAM ? a.sw.f0 : 0, t1 = SESS ? a.rows[ul].m1 : STREAM ? a.f1 : T;
+    if (SESS && t0 >= t1) return;
     const float* A = a.mag + (long long)ul * pitch * kFPad + f;
     float* M = a.m0 + (long long)ul * pitch * kFPad + f;
     if (f >= kF) {

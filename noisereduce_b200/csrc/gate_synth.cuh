@@ -106,7 +106,10 @@ __device__ __forceinline__ void k2c_freq_taps(const unsigned char* rows, unsigne
 #endif
 // STREAM (kMaskF32, b200gate_tstream_*): spectra and masks come from the stream's rings (K2Args::sw); the hops of a
 // launch are [pad / H + 2, ...) through Geom as usual, with y the virtual base of output sample `pad`.
-template <int HR, int MK, typename T, bool ROWS = false, bool STREAM = false>
+// SESS (with STREAM): each row's own hops [ha, hb) -- the same view with pad = (ha - 2) H and the span ending at
+// (hb - 2) H -- its bound min(T, hb + 1), and its output at y + rows[ul].y (global sample index; Geom's pad and n_total
+// are unused).
+template <int HR, int MK, typename T, bool ROWS = false, bool STREAM = false, bool SESS = false>
 __global__ void __launch_bounds__(kThreads, B200_K2C_MINBLOCKS) k2c_synthesize(const K2Args a) {
     constexpr int NH = 32 / HR;             // frames overlapping one hop (win / hop)
     constexpr int MB = k2c_mask_bytes<MK>();
@@ -157,15 +160,18 @@ __global__ void __launch_bounds__(kThreads, B200_K2C_MINBLOCKS) k2c_synthesize(c
         const int u = g.u0 + ul;
         const int ic = u / g.C, c = u - ic * g.C;
         const UnitDesc* ud = ROWS ? a.units + u : nullptr;           // ROWS: the unit's own span and frames
-        const long long i1 = ROWS ? ud->i1 : (long long)ic * g.step - g.pad;
-        long long out_len = ROWS ? ud->o_hi - ud->o_lo : g.n_total - (long long)ic * g.step;
-        if (!ROWS && out_len > g.step) out_len = g.step;
-        const int T_u = ROWS ? ud->T : g.T;                          // (g.T stays the pitch of the per-unit buffers)
-        long long jp_hi = g.pad + out_len;
+        const SessRow* sr = SESS ? a.rows + ul : nullptr;            // SESS: the row's own hops
+        const long long pad_s = SESS ? (long long)(sr->ha - 2) * H : 0;
+#define B200_K2C_PAD (SESS ? pad_s : g.pad)
+        const long long i1 = ROWS ? ud->i1 : SESS ? 0 : (long long)ic * g.step - g.pad;
+        long long out_len = ROWS ? ud->o_hi - ud->o_lo : SESS ? (long long)(sr->hb - sr->ha) * H : g.n_total - (long long)ic * g.step;
+        if (!ROWS && !SESS && out_len > g.step) out_len = g.step;
+        const int T_u = ROWS ? ud->T : SESS ? min(sr->T, sr->hb + 1) : g.T;   // (g.T stays the pitch of the per-unit buffers)
+        long long jp_hi = B200_K2C_PAD + out_len;
         const long long sig_len = (long long)(T_u - 1) * H;          // istft output length
         if (jp_hi > sig_len) jp_hi = sig_len;                        // beyond it the reference leaves zeros
-        if (jp_hi <= g.pad) continue;
-        const long long jlo = g.pad + kN / 2, jhi = jp_hi + kN / 2;
+        if (jp_hi <= B200_K2C_PAD) continue;
+        const long long jlo = B200_K2C_PAD + kN / 2, jhi = jp_hi + kN / 2;
         const int h_lo = (int)(jlo / H), h_hi = (int)((jhi + H - 1) / H);
         // ROWS: the recording's own work-item length.  A work item that ends on an odd frame transforms its last frame
         // alone instead of packed with its successor, which rounds differently in the last bit, so the hops at work-item
@@ -176,7 +182,8 @@ __global__ void __launch_bounds__(kThreads, B200_K2C_MINBLOCKS) k2c_synthesize(c
         if (hs >= he) continue;
         const int t_start = max(0, hs - (NH - 1)) & ~1;              // k1 packed frames (2j, 2j+1): walk the same pairs
         const int t_last = min(he - 1, T_u - 1);
-        T* yrow = ROWS ? static_cast<T*>(a.units[u].y) : static_cast<T*>(a.y) + (long long)c * g.out_stride;
+        T* yrow = ROWS ? static_cast<T*>(a.units[u].y) : SESS ? static_cast<T*>(a.y) + sr->y
+                                                       : static_cast<T*>(a.y) + (long long)c * g.out_stride;
         const float2* zunit = a.zcache + (long long)ul * a.zpairs * 1024;
         const unsigned short* munit = (MK == kMaskF32 || kBits) ? nullptr : a.num + (long long)ul * a.zpairs * (2 * kFPad);
         const float* funit = (MK == kMaskF32) ? a.fmask + (long long)ul * (STREAM ? a.sw.ring : g.T) * kFPad : nullptr;
@@ -415,7 +422,7 @@ __global__ void __launch_bounds__(kThreads, B200_K2C_MINBLOCKS) k2c_synthesize(c
             // hops t and t+1 are now complete (all frames <= t+1 have been added)
             {
                 const long long jp0 = (long long)t * H - kN / 2;             // chunk-local index of row 0, lane 0
-                if (t >= hs && t + 1 < he && t >= NH - 1 && t + 1 <= T_u - 1 && jp0 >= g.pad &&
+                if (t >= hs && t + 1 < he && t >= NH - 1 && t + 1 <= T_u - 1 && jp0 >= B200_K2C_PAD &&
                     jp0 + 2 * H <= jp_hi) {
                     // both hops interior and fully inside the chunk centre: 2*HR coalesced row stores
                     T* dst = yrow + i1 + jp0 + lane;
@@ -432,7 +439,7 @@ __global__ void __launch_bounds__(kThreads, B200_K2C_MINBLOCKS) k2c_synthesize(c
                         if (hop < hs || hop >= he) continue;
                         const int ro = (r % HR) * 32 + lane;
                         const long long jp = (long long)hop * H + ro - kN / 2;   // chunk-local output index
-                        if (jp < g.pad || jp >= jp_hi) continue;
+                        if (jp < B200_K2C_PAD || jp >= jp_hi) continue;
                         float inv;
                         if (hop >= NH - 1 && hop <= T_u - 1) {
                             inv = a.tb.invn[ro];
@@ -458,5 +465,6 @@ __global__ void __launch_bounds__(kThreads, B200_K2C_MINBLOCKS) k2c_synthesize(c
         }
     }
 }
+#undef B200_K2C_PAD
 
 }  // namespace b200

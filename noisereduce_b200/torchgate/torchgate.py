@@ -253,42 +253,30 @@ class TorchGate(torch.nn.Module):
         rows.  See TorchGateStream."""
         return TorchGateStream(self, n_rows, _lib)
 
+    def sessions(self, n_rows: int, _lib=None) -> "TorchGateSessions":
+        """Gate many live sessions in one stream of n_rows rows, each row starting, receiving samples and ending at its
+        own pace: the non-stationary gate, each session bit-identical to forward() on its own samples.  See
+        TorchGateSessions."""
+        return TorchGateSessions(self, n_rows, _lib)
 
-class TorchGateStream:
-    """The non-stationary TorchGate on rows that arrive block by block (TorchGate.stream(n_rows)).
 
-    push(block) takes a [n_rows, n] CUDA tensor (any n >= 0) and returns the [n_rows, m] output samples that have become
-    final; finish() returns the rest.  torch.cat of everything returned, along dim 1, equals tg(x) in every bit, where x
-    is the concatenation of the blocks, however x is cut into blocks.  The rows advance together.
-
-    Every stage of the gate looks ahead a bounded distance (stft frames n_fft / 2 samples, the moving mean `right`
-    frames, the smoothing nt frames, the overlap-add one window), so after R samples per row exactly
-        samples_returned = hop * max(0, hb - 2),   hb = 2 floor(nS / 2),   nS = 2 floor(c / 2) - 1 - right - nt,
-        c = floor((R - n_fft / 2) / hop) + 1
-    have been returned (right = n - 1 - (n - 1) // 2 for n = n_movemean_nonstationary, nt the smoothing's time extent in
-    frames, 0 without smoothing; frames are analysed and synthesised in pairs).  The most samples held back is
-        latency_samples = n_fft / 2 + hop * (right + nt + 4 + e) - 1,   e = 1 if right + nt is even, else 0
-    (4863 samples, 0.304 s, at 16 kHz with the defaults).
-
-    push() enqueues on the current CUDA stream of the blocks' device and never waits for the device; keep the pushes of a
-    stream on one CUDA stream.  The stream has its own library handle, made at the first push on that block's device and
-    released by finish() (releasing it waits for the device, as destroying any handle does).  The TorchGate's attributes
-    are read once, by stream().  Covered: the non-stationary gate at n_fft = win_length = 1024, hop 256, float32 /
-    float16 / bfloat16 blocks (the output has the block's dtype), smoothing extents the lengths= form of forward()
-    runs; other settings raise NotImplementedError, before any library handle is made."""
+class _LiveGate:
+    """What TorchGate.stream() and TorchGate.sessions() share: the refusals, the closed-form counts, the library handle
+    and the checks of a block.  _api / _cls name the public call and class in messages."""
+    _api, _cls = "TorchGate.stream()", "TorchGateStream"
 
     def __init__(self, tg: "TorchGate", n_rows: int, _lib=None):
         if not tg.nonstationary:
-            raise NotImplementedError("TorchGate.stream() needs nonstationary=True: the stationary gate's top_db floor and "
+            raise NotImplementedError(f"{self._api} needs nonstationary=True: the stationary gate's top_db floor and "
                                       "thresholds are taken over all of a row's frames, so no sample is final before the end")
         if not tg._tuned():
-            raise NotImplementedError("TorchGate.stream() needs the default STFT geometry (n_fft = win_length = 1024, "
+            raise NotImplementedError(f"{self._api} needs the default STFT geometry (n_fft = win_length = 1024, "
                                       f"hop_length = 256), not n_fft={tg.n_fft}, win_length={tg.win_length}, "
                                       f"hop_length={tg.hop_length}")
         nf, nt = tg._extents if tg.smoothing_filter is not None else (0, 0)
         reason = _rows_smoothing_refusal(nf, nt, True)
         if reason:
-            raise NotImplementedError(f"TorchGate.stream(): freq_mask_smooth_hz={tg.freq_mask_smooth_hz} / "
+            raise NotImplementedError(f"{self._api}: freq_mask_smooth_hz={tg.freq_mask_smooth_hz} / "
                                       f"time_mask_smooth_ms={tg.time_mask_smooth_ms} give smoothing extents ({nf}, {nt}) "
                                       f"bins / frames, {reason}")
         if isinstance(n_rows, bool) or not isinstance(n_rows, (int, np.integer)) or n_rows < 1:
@@ -303,11 +291,8 @@ class TorchGateStream:
         self._right, self._nt = n - 1 - (n - 1) // 2, nt
         e = 1 if (self._right + nt) % 2 == 0 else 0
         self.latency_samples = self._n_fft // 2 + self._hop * (self._right + nt + 4 + e) - 1
-        self.samples_received = 0
-        self.samples_returned = 0
         self._gate = None
         self._device = self._dtype = None
-        self._finished = False
 
     def returned_after(self, R: int) -> int:
         """samples_returned after R samples per row (the closed form above)."""
@@ -335,28 +320,61 @@ class TorchGateStream:
     def _stream(self):
         return torch.cuda.current_stream(self._device).cuda_stream if self._device.type == "cuda" else None
 
-    @torch.no_grad()
-    def push(self, block: torch.Tensor) -> torch.Tensor:
-        """Append block ([n_rows, n] samples of every row) and return the [n_rows, m] output samples now final."""
-        if self._finished:
-            raise ValueError("TorchGateStream.push() after finish()")
+    def _check_block(self, block):
         if not isinstance(block, torch.Tensor) or block.ndim != 2 or block.shape[0] != self.n_rows:
             shape = tuple(block.shape) if isinstance(block, torch.Tensor) else type(block).__name__
             raise ValueError(f"a block must be a [{self.n_rows}, n] tensor, got {shape}")
         if block.dtype == torch.float64:
-            raise NotImplementedError("TorchGateStream.push() takes float32 / float16 / bfloat16 blocks, not float64")
+            raise NotImplementedError(f"{self._cls}.push() takes float32 / float16 / bfloat16 blocks, not float64")
         if block.dtype not in (torch.float32, torch.float16, torch.bfloat16):
             raise ValueError(f"a block must be float32 / float16 / bfloat16, got {block.dtype}")
         if block.requires_grad:
-            raise NotImplementedError("TorchGateStream has no backward pass: push blocks that do not require grad")
+            raise NotImplementedError(f"{self._cls} has no backward pass: push blocks that do not require grad")
         if self._lib is None and not block.is_cuda:
-            raise ValueError("noisereduce_b200.TorchGateStream runs on CUDA tensors only (no CPU fallback)")
+            raise ValueError(f"noisereduce_b200.{self._cls} runs on CUDA tensors only (no CPU fallback)")
         if self._device is None:
             self._device, self._dtype = block.device, block.dtype
         elif block.device != self._device:
             raise ValueError(f"every block of a stream must be on {self._device}, got {block.device}")
         elif block.dtype != self._dtype:
             raise ValueError(f"every block of a stream must be {self._dtype}, got {block.dtype}")
+
+
+class TorchGateStream(_LiveGate):
+    """The non-stationary TorchGate on rows that arrive block by block (TorchGate.stream(n_rows)).
+
+    push(block) takes a [n_rows, n] CUDA tensor (any n >= 0) and returns the [n_rows, m] output samples that have become
+    final; finish() returns the rest.  torch.cat of everything returned, along dim 1, equals tg(x) in every bit, where x
+    is the concatenation of the blocks, however x is cut into blocks.  The rows advance together.
+
+    Every stage of the gate looks ahead a bounded distance (stft frames n_fft / 2 samples, the moving mean `right`
+    frames, the smoothing nt frames, the overlap-add one window), so after R samples per row exactly
+        samples_returned = hop * max(0, hb - 2),   hb = 2 floor(nS / 2),   nS = 2 floor(c / 2) - 1 - right - nt,
+        c = floor((R - n_fft / 2) / hop) + 1
+    have been returned (right = n - 1 - (n - 1) // 2 for n = n_movemean_nonstationary, nt the smoothing's time extent in
+    frames, 0 without smoothing; frames are analysed and synthesised in pairs).  The most samples held back is
+        latency_samples = n_fft / 2 + hop * (right + nt + 4 + e) - 1,   e = 1 if right + nt is even, else 0
+    (4863 samples, 0.304 s, at 16 kHz with the defaults).
+
+    push() enqueues on the current CUDA stream of the blocks' device and never waits for the device; keep the pushes of a
+    stream on one CUDA stream.  The stream has its own library handle, made at the first push on that block's device and
+    released by finish() (releasing it waits for the device, as destroying any handle does).  The TorchGate's attributes
+    are read once, by stream().  Covered: the non-stationary gate at n_fft = win_length = 1024, hop 256, float32 /
+    float16 / bfloat16 blocks (the output has the block's dtype), smoothing extents the lengths= form of forward()
+    runs; other settings raise NotImplementedError, before any library handle is made."""
+
+    def __init__(self, tg: "TorchGate", n_rows: int, _lib=None):
+        super().__init__(tg, n_rows, _lib)
+        self.samples_received = 0
+        self.samples_returned = 0
+        self._finished = False
+
+    @torch.no_grad()
+    def push(self, block: torch.Tensor) -> torch.Tensor:
+        """Append block ([n_rows, n] samples of every row) and return the [n_rows, m] output samples now final."""
+        if self._finished:
+            raise ValueError("TorchGateStream.push() after finish()")
+        self._check_block(block)
         n = block.shape[1]
         m = self.returned_after(self.samples_received + n) - self.samples_returned
         with self._ctx():
@@ -390,6 +408,143 @@ class TorchGateStream:
         self._finished = True
         self.samples_returned += m
         return y.to(dtype=self._dtype)
+
+
+class TorchGateSessions(_LiveGate):
+    """Many live sessions in one stream (TorchGate.sessions(n_rows)): every row holds its own session, which starts,
+    receives samples and ends at its own pace.
+
+    push(block, lengths) appends block[b, :lengths[b]] to row b's session for every row b (0 <= lengths[b] <= n for a
+    [n_rows, n] block) and returns (y, m): row b's new output is y[b, :m[b]], y is [n_rows, max(m)] in the block's dtype,
+    m a host list.  end(rows) ends the session in each listed row and returns its tail the same way (y[i, :m[i]] for
+    rows[i]); the row is then empty and its next samples start a new session.  reset(rows) drops the sessions in the
+    listed rows without output.  close() releases the library handle.
+
+    A session is the samples a row receives between its start (the creation of the object, or the end() / reset() that
+    last emptied the row) and its end().  For a session x_s of at least 2 * win_length samples, the concatenation of
+    everything returned for it, by pushes and by its end(), equals tg(x_s[None])[0] in every bit, however the session
+    was cut, whatever the other rows did meanwhile and whichever row it used.  After R samples of a session exactly
+    returned_after(R) of its output samples have been returned, and at most latency_samples are held back (the closed
+    forms of TorchGateStream).  samples_received / samples_returned are those counts for each row's current session.
+
+    push() and end() enqueue on the current CUDA stream of the blocks' device and never wait for the device, except that
+    the per-row tables travel through a ring of 16 pinned slots: a call waits when the device is 16 slices behind (a push
+    is one slice per 4096 samples of its longest row, an end() one).  Keep the calls of one object on one CUDA stream.
+    The library handle is made at the first push; its device memory is fixed then, by n_rows and the parameters, however
+    many sessions pass through.  close() waits for the device, as destroying any handle does.  Covered and refused as
+    TorchGate.stream(): NotImplementedError for other settings, before any library handle is made.  ValueError, before
+    any work: bad lengths (count, negative, larger than n, not integers), rows out of range or repeated, use after
+    close().  end() of a row holding fewer than 2 * win_length samples raises the reference's
+    Exception("x must be bigger than 2048") and changes no row."""
+    _api, _cls = "TorchGate.sessions()", "TorchGateSessions"
+
+    def __init__(self, tg: "TorchGate", n_rows: int, _lib=None):
+        super().__init__(tg, n_rows, _lib)
+        self._R = np.zeros(self.n_rows, dtype=np.int64)
+        self._E = np.zeros(self.n_rows, dtype=np.int64)
+        self._closed = False
+
+    @property
+    def samples_received(self) -> list:
+        return self._R.tolist()
+
+    @property
+    def samples_returned(self) -> list:
+        return self._E.tolist()
+
+    def _returned_after_rows(self, R: np.ndarray) -> np.ndarray:
+        """returned_after of every entry of R."""
+        c = (R - self._n_fft // 2) // self._hop + 1
+        nS = (c - c % 2) - 1 - self._right - self._nt
+        hb = nS - nS % 2
+        return np.where(R < self._n_fft // 2, 0, self._hop * np.maximum(0, hb - 2))
+
+    def _live(self, what):
+        if self._closed:
+            raise ValueError(f"TorchGateSessions.{what}() after close()")
+
+    def _ints(self, v, what):
+        """v as a 1-D int64 numpy array (a sequence of ints or a 1-D integer tensor)."""
+        if isinstance(v, torch.Tensor):
+            v = v.detach().cpu().numpy()                 # (a CUDA tensor: one device -> host copy)
+        try:
+            a = np.asarray(v)
+        except Exception:
+            a = None
+        if a is None or a.ndim != 1 or (a.size and a.dtype.kind not in "iu"):
+            raise ValueError(f"{what} must be a 1-D sequence of ints, got {v!r}")
+        return np.ascontiguousarray(a, dtype=np.int64)
+
+    def _rows(self, rows):
+        r = self._ints(rows, "rows")
+        if r.size and (r.min() < 0 or r.max() >= self.n_rows):
+            raise ValueError(f"rows out of range [0, {self.n_rows}): {r.tolist()}")
+        if np.unique(r).size != r.size:
+            raise ValueError(f"rows must not repeat, got {r.tolist()}")
+        return r
+
+    @torch.no_grad()
+    def push(self, block: torch.Tensor, lengths):
+        """Append block[b, :lengths[b]] to row b's session; returns (y, m), row b's new output being y[b, :m[b]]."""
+        self._live("push")
+        self._check_block(block)
+        n = self._ints(lengths, "lengths")
+        if n.size != self.n_rows:
+            raise ValueError(f"lengths has {n.size} entries, the stream has {self.n_rows} rows")
+        if n.size and (n.min() < 0 or n.max() > block.shape[1]):
+            raise ValueError(f"lengths must lie in [0, {block.shape[1]}] (the block's samples), got {n.tolist()}")
+        m = self._returned_after_rows(self._R + n) - self._E
+        m_max = int(m.max())
+        with self._ctx():
+            if self._gate is None:
+                self._open(block)
+            y = torch.empty((self.n_rows, m_max), dtype=torch.float32, device=self._device)
+            if n.max() > 0:
+                xf = block.detach().to(torch.float32).contiguous()
+                got = self._gate.tstream_push_rows(xf.data_ptr(), n, xf.stride(0), y.data_ptr() if m_max else None,
+                                                   max(m_max, 1), m_max, self._stream())
+                assert np.array_equal(got, m), (got, m)
+        self._R += n
+        self._E += m
+        return y.to(dtype=self._dtype), m.tolist()
+
+    @torch.no_grad()
+    def end(self, rows):
+        """End the sessions in rows; returns (y, m), the tail of rows[i] being y[i, :m[i]].  The rows are empty again."""
+        self._live("end")
+        r = self._rows(rows)
+        short = [int(b) for b in r if self._R[b] < 2 * self._win]
+        if short:
+            raise Exception(f"x must be bigger than {self._win * 2}")
+        m = (self._R[r] // self._hop) * self._hop - self._E[r]
+        m_max = int(m.max()) if m.size else 0
+        dtype = self._dtype or torch.float32
+        if not r.size:
+            return torch.empty((0, 0), dtype=dtype, device=self._device), []
+        with self._ctx():
+            y = torch.empty((r.size, m_max), dtype=torch.float32, device=self._device)
+            got = self._gate.tstream_end_rows(r, y.data_ptr() if m_max else None, max(m_max, 1), m_max, self._stream())
+            assert np.array_equal(got, m), (got, m)
+        self._R[r] = 0
+        self._E[r] = 0
+        return y.to(dtype=dtype), m.tolist()
+
+    def reset(self, rows):
+        """Drop the sessions in rows without output; the rows are empty again."""
+        self._live("reset")
+        r = self._rows(rows)
+        if self._gate is not None and r.size:
+            self._gate.tstream_reset_rows(r)
+        self._R[r] = 0
+        self._E[r] = 0
+
+    def close(self):
+        """Release the library handle (waits for the device).  Calling it again does nothing."""
+        if self._gate is not None:
+            with self._ctx():
+                self._gate.close()
+        self._gate = None
+        self._closed = True
 
 
 class _GateFunction(torch.autograd.Function):
