@@ -355,6 +355,30 @@ int b200gate_tstream_end_rows(b200gate_handle* h, const int64_t* rows, int64_t k
                               int64_t out_capacity, int64_t* n_out, void* cuda_stream);
 int b200gate_tstream_reset_rows(b200gate_handle* h, const int64_t* rows, int64_t k);
 
+/* ---- TorchGate.sessions(profiles=...): gate settings per row -------------------------------------------------------
+ * A profile is the part of the gate settings a row of a per-row stream may hold on its own; n_fft, win_length,
+ * hop_length and the gate type stay the handle's.  b200gate_tstream_set_profiles gives the handle's next streams the
+ * profiles p[0, k) (k >= 1); it is called before b200gate_tstream_begin, and without it a stream has one profile, the
+ * handle's own settings.  Every row starts on profile 0 and keeps its profile across sessions until
+ * b200gate_tstream_assign_rows puts rows[0, k) on another one; a row's session on profile j is bit-identical to
+ * b200gate_run on a handle whose settings are the handle's with profile j's, and hb(R) above uses that profile's
+ * n_movemean and n_grad_time.  The stream's device state is sized by the largest lookahead of its profiles.  Errors:
+ * B200GATE_ERR_ARG for k < 1, n_movemean < 1, negative extents, extents beyond the streaming smoothing (as
+ * b200gate_tstream_begin), prop_decrease outside [0, 1]; B200GATE_ERR_STATE while a torch stream is open.  assign:
+ * B200GATE_ERR_ARG for rows out of range or listed twice, a profile out of range, or a listed row whose session holds
+ * samples, and nothing changes.  The lockstep b200gate_tstream_push / _finish return B200GATE_ERR_STATE on a stream
+ * with more than one profile. */
+typedef struct b200gate_tprofile {
+    int32_t n_grad_freq;        /* smoothing half-widths; 0,0 = mask smoothing disabled                       */
+    int32_t n_grad_time;
+    int32_t n_movemean;
+    double thresh_n_mult;
+    double sigmoid_slope;       /* 1 / temp_coeff_nonstationary                                                 */
+    double prop_decrease;
+} b200gate_tprofile;
+int b200gate_tstream_set_profiles(b200gate_handle* h, const b200gate_tprofile* p, int64_t k);
+int b200gate_tstream_assign_rows(b200gate_handle* h, const int64_t* rows, int64_t k, int64_t profile);
+
 int b200gate_get_stats(const b200gate_handle* h, b200gate_stats* out);
 
 /* ---- sample formats of device-resident callers ----------------------------------------------------------------------

@@ -41,6 +41,7 @@ EXPORTS = [
     "b200gate_torch_apply_masks_rows", "b200gate_noise_stats_rows", "b200gate_set_noise_threshold_rows",
     "b200gate_tstream_begin", "b200gate_tstream_push", "b200gate_tstream_finish",
     "b200gate_tstream_push_rows", "b200gate_tstream_end_rows", "b200gate_tstream_reset_rows",
+    "b200gate_tstream_set_profiles", "b200gate_tstream_assign_rows",
 ]
 
 
@@ -80,6 +81,12 @@ class Row(C.Structure):
 class NoiseClip(C.Structure):
     """b200gate_noise_clip: one noise clip of b200gate_noise_stats_rows, [C][n] with row stride `stride` elements."""
     _fields_ = [("x", C.c_void_p), ("C", C.c_int64), ("n", C.c_int64), ("stride", C.c_int64)]
+
+
+class TProfile(C.Structure):
+    """b200gate_tprofile: the gate settings one row of a per-row torch stream may hold (b200gate_tstream_set_profiles)."""
+    _fields_ = [("n_grad_freq", C.c_int32), ("n_grad_time", C.c_int32), ("n_movemean", C.c_int32),
+                ("thresh_n_mult", C.c_double), ("sigmoid_slope", C.c_double), ("prop_decrease", C.c_double)]
 
 
 class GateError(RuntimeError):
@@ -154,6 +161,8 @@ class GateLibrary:
         d.b200gate_tstream_push_rows.argtypes = [vp, vp, C.POINTER(i64), i64, vp, i64, i64, C.POINTER(i64), vp]
         d.b200gate_tstream_end_rows.argtypes = [vp, C.POINTER(i64), i64, vp, i64, i64, C.POINTER(i64), vp]
         d.b200gate_tstream_reset_rows.argtypes = [vp, C.POINTER(i64), i64]
+        d.b200gate_tstream_set_profiles.argtypes = [vp, C.POINTER(TProfile), i64]
+        d.b200gate_tstream_assign_rows.argtypes = [vp, C.POINTER(i64), i64, i64]
 
 
 def _i64p(a: np.ndarray):
@@ -447,6 +456,14 @@ class Gate:
 
     def tstream_reset_rows(self, rows):
         self._check(self.lib.dll.b200gate_tstream_reset_rows(self._h, _i64p(rows), len(rows)))
+
+    def tstream_set_profiles(self, profiles):
+        """profiles: (n_grad_freq, n_grad_time, n_movemean, thresh_n_mult, sigmoid_slope, prop_decrease) tuples."""
+        arr = (TProfile * len(profiles))(*[TProfile(*p) for p in profiles])
+        self._check(self.lib.dll.b200gate_tstream_set_profiles(self._h, arr, len(profiles)))
+
+    def tstream_assign_rows(self, rows, profile):
+        self._check(self.lib.dll.b200gate_tstream_assign_rows(self._h, _i64p(rows), len(rows), profile))
 
     def set_range(self, mode: int, a: int = 0, b: int = 0):
         self._check(self.lib.dll.b200gate_set_range(self._h, mode, a, b))

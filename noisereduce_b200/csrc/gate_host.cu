@@ -144,9 +144,15 @@ struct b200gate_handle {
     // k of d_sess on the caller's stream, and ev_sess[k] marks that copy.  A slice waits for its slot's previous copy only,
     // so the host runs at most kSessSlots slices ahead of the device.  ts_mode: 0 until the first push, then 1 for the
     // lockstep calls or 2 for the per-row calls; a stream takes one kind only.
-    struct TsRow { long long R = 0, lo = 0, nA = 0, nM = 0, nS = 0, ha = 2; };
+    // Each row is gated with its profile (TsRow::prof) of ts_prof: the profiles b200gate_tstream_set_profiles gave
+    // (ts_prof_set), or the handle's own settings, fixed by b200gate_tstream_begin; d_prof is their device table.
+    // ts_sspan[j]: the largest smoothing span of a profile-j row in the slice being built (one smoothing launch each).
+    struct TsRow { long long R = 0, lo = 0, nA = 0, nM = 0, nS = 0, ha = 2; int prof = 0; };
     int ts_mode = 0;
     std::vector<TsRow> ts_row;
+    std::vector<b200gate_tprofile> ts_prof_set, ts_prof;
+    std::vector<long long> ts_sspan;
+    TsProfile* d_prof = nullptr;
     std::vector<long long> ts_y0;                  // b200gate_tstream_push_rows: each row's output offset in the call
     SessRow* hp_sess = nullptr;
     size_t hp_sess_bytes = 0;
@@ -3483,11 +3489,12 @@ int b200gate_stream_finish(b200gate_handle* h, void* out, int64_t out_stride, in
 // equals b200gate_run on the whole rows in every bit; b200gate_tstream_finish does the last frames with T = R / H + 1.
 namespace {
 
-long long ts_hops_done(const b200gate_handle* h, long long R) {      // hb(R) above
-    const int n = h->p.n_movemean, right = n - 1 - (n - 1) / 2;
+// A row gated with profile q (the moving mean's right reach and the smoothing's time extent are q's).
+long long ts_hops_done(const b200gate_handle* h, const b200gate_tprofile& q, long long R) {      // hb(R) above
+    const int n = q.n_movemean, right = n - 1 - (n - 1) / 2;
     if (R < kN / 2) return 2;
     const long long c = (R - kN / 2) / h->p.hop_length + 1;
-    const long long nS = (c & ~1LL) - 1 - right - h->p.n_grad_time;
+    const long long nS = (c & ~1LL) - 1 - right - q.n_grad_time;
     return std::max(2LL, nS & ~1LL);
 }
 
@@ -3495,27 +3502,40 @@ long long ts_hops_done(const b200gate_handle* h, long long R) {      // hb(R) ab
 // and smoothing done so far (nM0, nS0) and the first hop not yet returned (ha0): analysis to nA, moving mean to nM,
 // smoothing to nS, synthesis to hop hb.
 struct TsTarget { long long nA, nM, nS, hb; };
-TsTarget ts_target(const b200gate_handle* h, long long R, long long T, long long nM0, long long nS0, long long ha0) {
+TsTarget ts_target(const b200gate_handle* h, const b200gate_tprofile& q, long long R, long long T, long long nM0,
+                   long long nS0, long long ha0) {
     if (T > 0) return {T, T, T, T + 1};
-    const int n = h->p.n_movemean, right = n - 1 - (n - 1) / 2;
+    const int n = q.n_movemean, right = n - 1 - (n - 1) / 2;
     const long long c = R >= kN / 2 ? (R - kN / 2) / h->p.hop_length + 1 : 0;
-    const long long nA = c & ~1LL, nM = std::max(nM0, nA - 1 - right), nS = std::max(nS0, nM - h->p.n_grad_time);
+    const long long nA = c & ~1LL, nM = std::max(nM0, nA - 1 - right), nS = std::max(nS0, nM - q.n_grad_time);
     return {nA, nM, nS, std::max(ha0, nS & ~1LL)};
+}
+
+// Why the streaming smoothing cannot hold extents (nf, nt), or nullptr: the ring of 2 nt + 1 mask rows of k_smooth_box
+// (1 <= nf <= 12) or k_smooth_stream must fit shared memory.
+const char* ts_smoothing_refusal(int nf, int nt) {
+    if (nf < 0 || nt < 0) return "negative smoothing extents";
+    if (nf > 65535 || nt > 65535) return "beyond the shared-memory ring of the streaming smoothing";
+    const bool box = nf >= 1 && nf <= 12 && smoothb_smem_bytes(kFPad, nt) <= 200 * 1024;
+    if (!box && smooths_smem_bytes(kFPad, nf, nt) > 200 * 1024) return "beyond the shared-memory ring of the streaming smoothing";
+    return nullptr;
 }
 
 // The launches of one slice: frames [a0, a1) of analysis, [m0, m1) of moving mean, [s0, s1) of smoothing and hops
 // [ha, hb) of synthesis, under the frame bound Tb (INT_MAX while the end is unknown), R samples in the window x (the
 // virtual base of sample 0), hop ha's first sample to out[b][0].  SESS: every row's ranges, bound, window start and
 // output offset come from the device table `rows`; the ranges here start at 0 and end at the largest span of any row,
-// which sizes the grids (rows with less to do leave early), and Tb, R and x are unused.
+// which sizes the grids (rows with less to do leave early), and Tb, R and x are unused.  SESS smooths in one launch per
+// profile whose rows have frames to smooth (h->ts_sspan), each with that profile's extents.
 struct TsSlice { long long a0, a1, m0, m1, s0, s1, ha, hb; int Tb; long long R; const float* x; };
 
 extern "C++" {                                             // (this file's entry points have C linkage)
 template <bool SESS>
 int ts_launch(b200gate_handle* h, const TsSlice& s, const SessRow* rows, float* out, long long out_stride, cudaStream_t st) {
     const b200gate_params& p = h->p;
-    const int H = p.hop_length, nt = p.n_grad_time, nf = p.n_grad_freq, ring = h->ts_ring;
-    const int n = p.n_movemean;
+    const b200gate_tprofile& q = h->ts_prof[0];              // (the lockstep calls take one profile only)
+    const int H = p.hop_length, nt = q.n_grad_time, nf = q.n_grad_freq, ring = h->ts_ring;
+    const int n = q.n_movemean;
     const int B = (int)h->ts_B;
     const Tables tb = device_tables(h);
     StreamWin sw{};
@@ -3536,19 +3556,22 @@ int ts_launch(b200gate_handle* h, const TsSlice& s, const SessRow* rows, float* 
     }
     if (s.m1 > s.m0) {
         TMovArgs ma{};
-        ma.n_units = B; ma.T = s.Tb; ma.n_movemean = n; ma.n_thresh = (float)p.thresh_n_mult;
-        ma.inv_temp = (float)p.sigmoid_slope; ma.p = (float)p.prop_decrease; ma.mag = h->d_ts_mag; ma.m0 = h->d_ts_m0;
+        ma.n_units = B; ma.T = s.Tb; ma.n_movemean = n; ma.n_thresh = (float)q.thresh_n_mult;
+        ma.inv_temp = (float)q.sigmoid_slope; ma.p = (float)q.prop_decrease; ma.mag = h->d_ts_mag; ma.m0 = h->d_ts_m0;
         sw.f0 = (int)s.m0;
-        ma.sw = sw; ma.f1 = (int)s.m1; ma.run = h->d_ts_run; ma.rows = rows;
+        ma.sw = sw; ma.f1 = (int)s.m1; ma.run = h->d_ts_run; ma.rows = rows; ma.prof = h->d_prof;
         auto kern_ = k_tgate_movmean<false, true, SESS>;
         B200_LAUNCH(kern_, dim3(grid_1d((long long)B * kFPad, 128, 1 << 30)), dim3(128), 0, st, ma);
     }
-    if (s.s1 > s.s0) {
+    for (size_t j = 0; j < (SESS ? h->ts_prof.size() : 1); ++j) {
+        const long long s0 = SESS ? 0 : s.s0, s1 = SESS ? h->ts_sspan[j] : s.s1;
+        if (s1 <= s0) continue;
+        const int nfj = h->ts_prof[j].n_grad_freq, ntj = h->ts_prof[j].n_grad_time;
         SmoothFArgs sa{};
-        sa.n_units = B; sa.T = s.Tb; sa.nf = nf; sa.nt = nt; sa.tf_lo = (int)s.s0; sa.tf_hi = (int)s.s1; sa.F = kF; sa.FPad = kFPad;
+        sa.n_units = B; sa.T = s.Tb; sa.nf = nfj; sa.nt = ntj; sa.tf_lo = (int)s0; sa.tf_hi = (int)s1; sa.F = kF; sa.FPad = kFPad;
         sa.p = 1.0f; sa.one_minus_p = 0.0f;                  // (the torch surface blends in k_tgate_movmean)
-        sa.m0 = h->d_ts_m0; sa.m2 = h->d_ts_mask; sa.sw = sw; sa.rows = rows;
-        launch_smooth_float<false, true, SESS>(sa, nf, nt, (int)s.s0, (int)s.s1, B, 0, st);   // (extents checked at begin)
+        sa.m0 = h->d_ts_m0; sa.m2 = h->d_ts_mask; sa.sw = sw; sa.rows = rows; sa.prof = (int)j;
+        launch_smooth_float<false, true, SESS>(sa, nfj, ntj, (int)s0, (int)s1, B, 0, st);   // (extents checked at begin)
     }
     if (s.hb > s.ha) {
         // hops [ha, hb): Geom's padded-chunk view with pad = (ha - 2) H puts the first of them at h_lo and output sample
@@ -3579,7 +3602,7 @@ int ts_launch(b200gate_handle* h, const TsSlice& s, const SessRow* rows, float* 
 // moving mean, smoothing, synthesis of what has become final.  The hops returned go to out[b][0, ...) (row stride
 // out_stride).
 int ts_advance(b200gate_handle* h, long long T, float* out, long long out_stride, cudaStream_t st) {
-    const TsTarget t = ts_target(h, h->ts_R, T, h->ts_nM, h->ts_nS, h->ts_ha);
+    const TsTarget t = ts_target(h, h->ts_prof[0], h->ts_R, T, h->ts_nM, h->ts_nS, h->ts_ha);
     const TsSlice s{h->ts_nA, t.nA, h->ts_nM, t.nM, h->ts_nS, t.nS, h->ts_ha, t.hb, T > 0 ? (int)T : INT_MAX, h->ts_R,
                     h->d_ts_win - h->ts_lo};
     const int rc = ts_launch<false>(h, s, nullptr, out, out_stride, st);
@@ -3597,6 +3620,7 @@ void ts_release(b200gate_handle* h) {
 
 const char* const kTsLockstep = "this torch stream advances its rows together (b200gate_tstream_push / _finish)";
 const char* const kTsPerRow = "this torch stream advances its rows one by one (b200gate_tstream_push_rows / _end_rows / _reset_rows)";
+const char* const kTsProfiles = "this torch stream gates its rows with several profiles (b200gate_tstream_push_rows / _end_rows)";
 
 // The per-row calls: an open stream that has not taken the lockstep calls.
 int sess_check(b200gate_handle* h) {
@@ -3618,15 +3642,23 @@ int sess_check_rows(b200gate_handle* h, const int64_t* rows, int64_t k) {
 }
 
 // Row r's table entry for a slice that brings it to r.R samples (T = 0) or ends it (T = R / H + 1); its output sample j
-// goes to out[y + j].  Advances r and widens the largest spans in `span`.
-void sess_fill(const b200gate_handle* h, b200gate_handle::TsRow& r, SessRow& e, long long T, long long y, TsSlice& span) {
-    const TsTarget t = ts_target(h, r.R, T, r.nM, r.nS, r.ha);
-    e.R = r.R; e.lo = r.lo; e.y = y; e.T = T > 0 ? (int)T : INT_MAX;
+// goes to out[y + j].  Advances r and widens the largest spans in `span` (the smoothing's in h->ts_sspan, per profile).
+void sess_fill(b200gate_handle* h, b200gate_handle::TsRow& r, SessRow& e, long long T, long long y, TsSlice& span) {
+    const TsTarget t = ts_target(h, h->ts_prof[r.prof], r.R, T, r.nM, r.nS, r.ha);
+    e.R = r.R; e.lo = r.lo; e.y = y; e.T = T > 0 ? (int)T : INT_MAX; e.prof = r.prof;
     e.a0 = (int)r.nA; e.a1 = (int)t.nA; e.m0 = (int)r.nM; e.m1 = (int)t.nM;
     e.s0 = (int)r.nS; e.s1 = (int)t.nS; e.ha = (int)r.ha; e.hb = (int)t.hb;
     span.a1 = std::max(span.a1, t.nA - r.nA); span.m1 = std::max(span.m1, t.nM - r.nM);
     span.s1 = std::max(span.s1, t.nS - r.nS); span.hb = std::max(span.hb, t.hb - r.ha);
+    h->ts_sspan[r.prof] = std::max(h->ts_sspan[r.prof], t.nS - r.nS);
     r.nA = t.nA; r.nM = t.nM; r.nS = t.nS; r.ha = t.hb;
+}
+
+// Empty row r: its next samples start a new session, on the profile it holds.
+void sess_empty(b200gate_handle::TsRow& r) {
+    const int prof = r.prof;
+    r = b200gate_handle::TsRow{};
+    r.prof = prof;
 }
 
 // The next slot of the upload ring; waits for that slot's previous copy to have left it (the only wait of the per-row
@@ -3637,6 +3669,7 @@ SessRow* sess_slot(b200gate_handle* h, int* k) {
     SessRow* tab = h->hp_sess + (size_t)*k * h->ts_B;
     memset(tab, 0, (size_t)h->ts_B * sizeof(SessRow));
     for (long long b = 0; b < h->ts_B; ++b) { tab[b].ha = tab[b].hb = 2; tab[b].T = INT_MAX; }   // (nothing to do)
+    std::fill(h->ts_sspan.begin(), h->ts_sspan.end(), 0LL);
     return tab;
 }
 
@@ -3666,21 +3699,30 @@ int b200gate_tstream_begin(b200gate_handle* h, int64_t n_rows) {
                     "= 1024, hop_length = 256 (the stationary gate's statistics span the whole row)");
     if (h->s_open) return fail(h, B200GATE_ERR_STATE, "a stream is open on this handle (b200gate_stream_finish first)");
     if (n_rows <= 0 || n_rows > 0x7fffffffLL / kFPad) return fail(h, B200GATE_ERR_ARG, "bad argument");
-    const int nf = p.n_grad_freq, nt = p.n_grad_time;
-    const bool box = nf >= 1 && nf <= 12 && smoothb_smem_bytes(kFPad, nt) <= 200 * 1024;
-    if (!box && smooths_smem_bytes(kFPad, nf, nt) > 200 * 1024)
-        return fail(h, B200GATE_ERR_ARG, "smoothing extents (%d, %d) beyond the shared-memory ring of the streaming smoothing",
-                    nf, nt);
-    ts_release(h);
-    const int n = p.n_movemean, left = (n - 1) / 2, right = n - 1 - left;
+    std::vector<b200gate_tprofile> prof = h->ts_prof_set;
+    if (prof.empty())
+        prof.push_back(b200gate_tprofile{p.n_grad_freq, p.n_grad_time, p.n_movemean, p.thresh_n_mult, p.sigmoid_slope,
+                                         p.prop_decrease});
     // A push is consumed in slices of S samples: a slice adds at most S / H + 2 frames to each stage.  Frames live in the
     // rings from their analysis until the last stage reads them: the moving mean reads |X| from nM - left to nA, the
     // smoothing masks from nS - nt to nM, the synthesis spectra and masks from hop ha - 4 (<= nS - 5) on.  Between
-    // slices nA - nM <= right + 1 and nM - nS <= nt, so left + right + 2 nt + S / H + 8 frames always suffice.
+    // slices nA - nM <= right + 1 and nM - nS <= nt, so left + right + 2 nt + S / H + 8 frames always suffice -- for
+    // every row with its own profile's left, right and nt, so the largest over the profiles sizes the rings.
     const long long S = 4096;
-    long long need = left + right + 2LL * nt + S / 256 + 16, ring = 16;
+    for (const b200gate_tprofile& q : prof) {
+        const char* why = ts_smoothing_refusal(q.n_grad_freq, q.n_grad_time);
+        if (why) return fail(h, B200GATE_ERR_ARG, "smoothing extents (%d, %d) %s", q.n_grad_freq, q.n_grad_time, why);
+    }
+    ts_release(h);
+    long long need = 0, ring = 16;
+    int n_max = 0;
+    for (const b200gate_tprofile& q : prof) {
+        const long long n = q.n_movemean, left = (n - 1) / 2, right = n - 1 - left;
+        need = std::max(need, left + right + 2LL * q.n_grad_time + S / 256 + 16);
+        n_max = std::max(n_max, q.n_movemean);
+    }
     while (ring < need) ring *= 2;
-    if (ring > (1 << 20)) return fail(h, B200GATE_ERR_ARG, "n_movemean %d: frame rings too large", n);
+    if (ring > (1 << 20)) return fail(h, B200GATE_ERR_ARG, "n_movemean %d: frame rings too large", n_max);
     // the sample window keeps [nA H - n_fft / 2, R) (< 2 H + n_fft samples) before a slice; with a pitch of
     // S + 2 (2 H + n_fft) a compaction never moves a span onto itself
     const long long cap = S + 2 * (2 * 256 + kN);
@@ -3689,7 +3731,8 @@ int b200gate_tstream_begin(b200gate_handle* h, int64_t n_rows) {
     const size_t o_win = 0, o_z = o_win + al(B * cap * 4), o_mag = o_z + al(B * (size_t)(ring / 2) * 1024 * 8);
     const size_t o_m0 = o_mag + al(B * ring * kFPad * 4), o_mask = o_m0 + al(B * ring * kFPad * 4);
     const size_t o_run = o_mask + al(B * ring * kFPad * 4), o_sess = o_run + al(B * kFPad * 8);
-    const size_t sess_bytes = (size_t)kSessSlots * B * sizeof(SessRow), bytes = o_sess + al(sess_bytes);
+    const size_t sess_bytes = (size_t)kSessSlots * B * sizeof(SessRow), o_prof = o_sess + al(sess_bytes);
+    const size_t bytes = o_prof + al(prof.size() * sizeof(TsProfile));
     if (h->ev_sess.empty()) {
         h->ev_sess.assign(kSessSlots, nullptr);
         for (cudaEvent_t& ev : h->ev_sess) CK(h, cudaEventCreateWithFlags(&ev, cudaEventDisableTiming));
@@ -3709,6 +3752,17 @@ int b200gate_tstream_begin(b200gate_handle* h, int64_t n_rows) {
     h->d_ts_win = (float*)(base + o_win); h->d_ts_z = (float2*)(base + o_z); h->d_ts_mag = (float*)(base + o_mag);
     h->d_ts_m0 = (float*)(base + o_m0); h->d_ts_mask = (float*)(base + o_mask); h->d_ts_run = (double*)(base + o_run);
     h->d_sess = (SessRow*)(base + o_sess);
+    h->d_prof = (TsProfile*)(base + o_prof);
+    std::vector<TsProfile> tab;                                // the floats of b200gate_run's k_tgate_movmean arguments
+    for (const b200gate_tprofile& q : prof)
+        tab.push_back(TsProfile{q.n_movemean, (float)q.thresh_n_mult, (float)q.sigmoid_slope, (float)q.prop_decrease});
+    e = cudaMemcpy(h->d_prof, tab.data(), tab.size() * sizeof(TsProfile), cudaMemcpyHostToDevice);
+    if (e != cudaSuccess) {
+        ts_release(h);
+        return fail(h, B200GATE_ERR_CUDA, "profile table upload: %s", cudaGetErrorString(e));
+    }
+    h->ts_prof = prof;
+    h->ts_sspan.assign(prof.size(), 0);
     h->ts_row.assign(B, b200gate_handle::TsRow{});
     h->ts_y0.assign(B, 0);
     h->ts_B = n_rows; h->ts_R = 0; h->ts_lo = 0; h->ts_cap = cap; h->ts_slice = S; h->ts_ring = (int)ring;
@@ -3725,8 +3779,9 @@ int b200gate_tstream_push(b200gate_handle* h, const float* in, int64_t n, int64_
         (h->ts_B > 1 && out_stride < out_capacity))
         return fail(h, B200GATE_ERR_ARG, "bad argument");
     if (h->ts_mode == 2) return fail(h, B200GATE_ERR_STATE, kTsPerRow);
+    if (h->ts_prof.size() > 1) return fail(h, B200GATE_ERR_STATE, kTsProfiles);
     const long long H = h->p.hop_length;
-    const long long m = (ts_hops_done(h, h->ts_R + n) - h->ts_ha) * H;
+    const long long m = (ts_hops_done(h, h->ts_prof[0], h->ts_R + n) - h->ts_ha) * H;
     if (out_capacity < m)
         return fail(h, B200GATE_ERR_ARG, "out_capacity %lld < %lld samples returned by this push", (long long)out_capacity, m);
     *n_out = m;
@@ -3763,6 +3818,7 @@ int b200gate_tstream_finish(b200gate_handle* h, float* out, int64_t out_stride, 
     if (!n_out || out_capacity < 0 || (out_capacity > 0 && !out) || (h->ts_B > 1 && out_stride < out_capacity))
         return fail(h, B200GATE_ERR_ARG, "bad argument");
     if (h->ts_mode == 2) return fail(h, B200GATE_ERR_STATE, kTsPerRow);
+    if (h->ts_prof.size() > 1) return fail(h, B200GATE_ERR_STATE, kTsProfiles);
     const long long H = h->p.hop_length, R = h->ts_R;
     if (R < 2 * h->p.win_length) return fail(h, B200GATE_ERR_ARG, "x must be bigger than %d", 2 * h->p.win_length);
     const long long T = R / H + 1, m = (T + 1 - h->ts_ha) * H;      // the rest of torch.istft's (T - 1) H samples
@@ -3786,12 +3842,16 @@ int b200gate_tstream_push_rows(b200gate_handle* h, const float* in, const int64_
     for (long long b = 0; b < B; ++b) {
         if (n[b] < 0) return fail(h, B200GATE_ERR_ARG, "row %lld: a negative sample count (%lld)", b, (long long)n[b]);
         n_max = std::max(n_max, (long long)n[b]);
-        m_max = std::max(m_max, (ts_hops_done(h, h->ts_row[b].R + n[b]) - h->ts_row[b].ha) * H);
+        const b200gate_handle::TsRow& r = h->ts_row[b];
+        m_max = std::max(m_max, (ts_hops_done(h, h->ts_prof[r.prof], r.R + n[b]) - r.ha) * H);
     }
     if (n_max > 0 && (!in || (B > 1 && in_stride < n_max))) return fail(h, B200GATE_ERR_ARG, "bad argument");
     if (out_capacity < m_max)
         return fail(h, B200GATE_ERR_ARG, "out_capacity %lld < %lld samples returned by this push", (long long)out_capacity, m_max);
-    for (long long b = 0; b < B; ++b) n_out[b] = (ts_hops_done(h, h->ts_row[b].R + n[b]) - h->ts_row[b].ha) * H;
+    for (long long b = 0; b < B; ++b) {
+        const b200gate_handle::TsRow& r = h->ts_row[b];
+        n_out[b] = (ts_hops_done(h, h->ts_prof[r.prof], r.R + n[b]) - r.ha) * H;
+    }
     h->ts_mode = 2;
     cudaStream_t st = (cudaStream_t)stream;
     std::vector<long long>& y0 = h->ts_y0;               // row b's output sample j goes to out[y0[b] + j] in this call
@@ -3854,7 +3914,7 @@ int b200gate_tstream_end_rows(b200gate_handle* h, const int64_t* rows, int64_t k
         b200gate_handle::TsRow& r = h->ts_row[rows[i]];
         n_out[i] = (r.R / H + 2 - r.ha) * H;
         sess_fill(h, r, tab[rows[i]], r.R / H + 1, i * out_stride - (r.ha - 2) * H, span);
-        r = b200gate_handle::TsRow{};                         // the row's next samples start a new session
+        sess_empty(r);
     }
     if ((rc = sess_submit(h, slot, span, nullptr, 0, 0, out, (cudaStream_t)stream))) ts_release(h);
     return rc;
@@ -3865,7 +3925,41 @@ int b200gate_tstream_reset_rows(b200gate_handle* h, const int64_t* rows, int64_t
     int rc;
     if ((rc = sess_check(h)) || (rc = sess_check_rows(h, rows, k))) return rc;
     h->ts_mode = 2;
-    for (int64_t i = 0; i < k; ++i) h->ts_row[rows[i]] = b200gate_handle::TsRow{};
+    for (int64_t i = 0; i < k; ++i) sess_empty(h->ts_row[rows[i]]);
+    return B200GATE_OK;
+}
+
+int b200gate_tstream_set_profiles(b200gate_handle* h, const b200gate_tprofile* p, int64_t k) {
+    if (!h) return B200GATE_ERR_ARG;
+    if (h->ts_open) return fail(h, B200GATE_ERR_STATE, "a torch stream is open (set the profiles before b200gate_tstream_begin)");
+    if (k < 1 || !p) return fail(h, B200GATE_ERR_ARG, "bad argument");
+    for (int64_t j = 0; j < k; ++j) {
+        const b200gate_tprofile& q = p[j];
+        const char* why = ts_smoothing_refusal(q.n_grad_freq, q.n_grad_time);
+        if (why)
+            return fail(h, B200GATE_ERR_ARG, "profile %lld: smoothing extents (%d, %d) %s", (long long)j, q.n_grad_freq,
+                        q.n_grad_time, why);
+        if (q.n_movemean < 1)
+            return fail(h, B200GATE_ERR_ARG, "profile %lld: n_movemean %d < 1", (long long)j, q.n_movemean);
+        if (!(q.prop_decrease >= 0.0 && q.prop_decrease <= 1.0))
+            return fail(h, B200GATE_ERR_ARG, "profile %lld: prop_decrease %g outside [0, 1]", (long long)j, q.prop_decrease);
+    }
+    h->ts_prof_set.assign(p, p + k);
+    return B200GATE_OK;
+}
+
+int b200gate_tstream_assign_rows(b200gate_handle* h, const int64_t* rows, int64_t k, int64_t profile) {
+    if (!h) return B200GATE_ERR_ARG;
+    int rc;
+    if ((rc = sess_check(h)) || (rc = sess_check_rows(h, rows, k))) return rc;
+    if (profile < 0 || profile >= (int64_t)h->ts_prof.size())
+        return fail(h, B200GATE_ERR_ARG, "profile %lld out of range [0, %zu)", (long long)profile, h->ts_prof.size());
+    for (int64_t i = 0; i < k; ++i)
+        if (h->ts_row[rows[i]].R > 0)
+            return fail(h, B200GATE_ERR_ARG, "row %lld holds a session of %lld samples (end or reset it first)",
+                        (long long)rows[i], h->ts_row[rows[i]].R);
+    h->ts_mode = 2;
+    for (int64_t i = 0; i < k; ++i) h->ts_row[rows[i]].prof = (int)profile;
     return B200GATE_OK;
 }
 

@@ -93,6 +93,14 @@ struct SessRow {
     int s0, s1;             // smoothing frames
     int ha, hb;             // synthesis hops [ha, hb), ha even
     int T;                  // the frame bound: INT_MAX while the session is live, R / H + 1 in the end() that finishes it
+    int prof;               // the row's gate settings: entry of the stream's profile table (TsProfile)
+};
+
+// The gate settings a SESS row is gated with (b200gate_tstream_set_profiles; one entry, the handle's own, without it).
+// k_tgate_movmean reads them per row; the smoothing extents select the smoothing launch (SmoothFArgs::prof).
+struct TsProfile {
+    int n_movemean;
+    float n_thresh, inv_temp, p;
 };
 
 struct SessCopyArgs {
@@ -1562,6 +1570,7 @@ struct SmoothFArgs {
                                // tf_hi the largest of the batch
     StreamWin sw;              // STREAM instantiations: m0 / m2 are rings of sw.ring rows; T bounds the frames only
     const SessRow* rows;       // SESS instantiations: row ul's frames [s0, s1) and bound T (tf_lo, tf_hi and T unused)
+    int prof;                  // SESS: the profile whose extents (nf, nt) this launch smooths; other rows leave at once
 };
 __host__ __device__ inline int smoothf_cpitch(int FPad, int nf) { return FPad + 2 * nf + 1; }
 inline size_t smoothf_smem_bytes(int TT, int FPad, int nf) { return (size_t)TT * smoothf_cpitch(FPad, nf) * 4; }
@@ -1621,6 +1630,7 @@ __global__ void __launch_bounds__(288) k_smooth_stream(const SmoothFArgs a) {
     float* row = s_buf + (size_t)R * FP;     // [nf | FP | nf]
     const int ul = blockIdx.y;
     const int T = ROWS ? a.units[ul].T : SESS ? a.rows[ul].T : a.T;
+    if (SESS && a.rows[ul].prof != a.prof) return;       // (smoothed by its own profile's launch)
     const int tf_hi = ROWS ? a.units[ul].tf_hi : SESS ? a.rows[ul].s1 : a.tf_hi;
     const int t_begin = (SESS ? a.rows[ul].s0 : a.tf_lo) + blockIdx.x * a.TT;
     if (t_begin >= tf_hi) return;
@@ -1693,6 +1703,7 @@ __global__ void __launch_bounds__(288) k_smooth_box(const SmoothFArgs a) {
     float* rowB = rowA + FP + 32;                          // [FP + 16]
     const int ul = blockIdx.y;
     const int T = ROWS ? a.units[ul].T : SESS ? a.rows[ul].T : a.T;
+    if (SESS && a.rows[ul].prof != a.prof) return;       // (smoothed by its own profile's launch)
     const int tf_hi = ROWS ? a.units[ul].tf_hi : SESS ? a.rows[ul].s1 : a.tf_hi;
     const int t_begin = (SESS ? a.rows[ul].s0 : a.tf_lo) + blockIdx.x * a.TT;
     if (t_begin >= tf_hi) return;
@@ -1912,13 +1923,15 @@ struct TMovArgs {
     int f1;
     double* run;               // STREAM: [n_units][FPad] the running sums, carried from one launch to the next
     const SessRow* rows;       // SESS instantiations: row ul's frames [m0, m1) and bound T (sw.f0, f1 and T unused)
+    const TsProfile* prof;     // SESS: the profile table; row ul's n_movemean, n_thresh, inv_temp and p are
+                               // prof[rows[ul].prof]'s (the four fields above unused)
 };
 
 // STREAM: frames [sw.f0, f1) of a stream whose rows have T frames (T = INT_MAX while the end is not known: the caller
 // then has |X| up to frame f1 + right).  The running sum is loaded from a.run, receives the same adds and subtracts in
 // the same order as the walk from t = 0 below, and is stored back, so its rounding is that of the whole-row walk.
 // SESS: the same per row; a session's first launch starts at frame 0 and builds the sum afresh, so a row that starts a
-// new session never reads the sum its previous session left.
+// new session never reads the sum its previous session left.  The gate settings are the row's profile's, read once.
 template <bool ROWS = false, bool STREAM = false, bool SESS = false>
 __global__ void __launch_bounds__(128) k_tgate_movmean(const TMovArgs a) {
     const long long idx = (long long)blockIdx.x * blockDim.x + threadIdx.x;
@@ -1934,8 +1947,11 @@ __global__ void __launch_bounds__(128) k_tgate_movmean(const TMovArgs a) {
         for (int t = t0; t < t1; ++t) M[(long long)(t & rmask) * kFPad] = 0.f;
         return;
     }
+    const TsProfile* pr = SESS ? a.prof + a.rows[ul].prof : nullptr;
+    const float n_thresh = SESS ? pr->n_thresh : a.n_thresh, inv_temp = SESS ? pr->inv_temp : a.inv_temp;
+    const float p = SESS ? pr->p : a.p;
     // conv1d(ones(n), padding="same"): window [t - left, t + right], zero padded, left = (n-1)/2
-    const int n = a.n_movemean, left = (n - 1) / 2, right = n - 1 - left;
+    const int n = SESS ? pr->n_movemean : a.n_movemean, left = (n - 1) / 2, right = n - 1 - left;
     double run = 0.0;
     if (t0 == 0) {
         for (int t = 0; t <= right && t < T; ++t) run += (double)A[(long long)(t & rmask) * kFPad];
@@ -1946,8 +1962,8 @@ __global__ void __launch_bounds__(128) k_tgate_movmean(const TMovArgs a) {
         const float Av = A[(long long)(t & rmask) * kFPad];
         const float S = (float)(run / (double)n);
         const float r = (Av - S) / S;
-        const float m = 1.0f / (1.0f + expf(-(r - a.n_thresh) * a.inv_temp));
-        M[(long long)(t & rmask) * kFPad] = a.p * (m - 1.0f) + 1.0f;
+        const float m = 1.0f / (1.0f + expf(-(r - n_thresh) * inv_temp));
+        M[(long long)(t & rmask) * kFPad] = p * (m - 1.0f) + 1.0f;
         const int tin = t + 1 + right, tout = t - left;
         if (tin < T) run += (double)A[(long long)(tin & rmask) * kFPad];
         if (tout >= 0) run -= (double)A[(long long)(tout & rmask) * kFPad];

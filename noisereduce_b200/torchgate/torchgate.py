@@ -253,19 +253,21 @@ class TorchGate(torch.nn.Module):
         rows.  See TorchGateStream."""
         return TorchGateStream(self, n_rows, _lib)
 
-    def sessions(self, n_rows: int, _lib=None) -> "TorchGateSessions":
+    def sessions(self, n_rows: int, profiles=None, _lib=None) -> "TorchGateSessions":
         """Gate many live sessions in one stream of n_rows rows, each row starting, receiving samples and ending at its
-        own pace: the non-stationary gate, each session bit-identical to forward() on its own samples.  See
-        TorchGateSessions."""
-        return TorchGateSessions(self, n_rows, _lib)
+        own pace: the non-stationary gate, each session bit-identical to forward() on its own samples.  profiles: a list
+        of dicts, each overriding some of this module's sample rate and gate strength for the rows put on it (see
+        TorchGateSessions).  See TorchGateSessions."""
+        return TorchGateSessions(self, n_rows, profiles, _lib)
 
 
 class _LiveGate:
     """What TorchGate.stream() and TorchGate.sessions() share: the refusals, the closed-form counts, the library handle
-    and the checks of a block.  _api / _cls name the public call and class in messages."""
+    and the checks of a block.  _api / _cls name the public call and class in messages.  profiles (sessions() only):
+    the dicts of TorchGateSessions, each checked as its own TorchGate; without them there is one profile, tg's own."""
     _api, _cls = "TorchGate.stream()", "TorchGateStream"
 
-    def __init__(self, tg: "TorchGate", n_rows: int, _lib=None):
+    def __init__(self, tg: "TorchGate", n_rows: int, _lib=None, profiles=None):
         if not tg.nonstationary:
             raise NotImplementedError(f"{self._api} needs nonstationary=True: the stationary gate's top_db floor and "
                                       "thresholds are taken over all of a row's frames, so no sample is final before the end")
@@ -273,33 +275,48 @@ class _LiveGate:
             raise NotImplementedError(f"{self._api} needs the default STFT geometry (n_fft = win_length = 1024, "
                                       f"hop_length = 256), not n_fft={tg.n_fft}, win_length={tg.win_length}, "
                                       f"hop_length={tg.hop_length}")
-        nf, nt = tg._extents if tg.smoothing_filter is not None else (0, 0)
-        reason = _rows_smoothing_refusal(nf, nt, True)
-        if reason:
-            raise NotImplementedError(f"{self._api}: freq_mask_smooth_hz={tg.freq_mask_smooth_hz} / "
-                                      f"time_mask_smooth_ms={tg.time_mask_smooth_ms} give smoothing extents ({nf}, {nt}) "
-                                      f"bins / frames, {reason}")
+        gates = [tg] if profiles is None else _profile_gates(tg, profiles)
+        where = (lambda k: "") if profiles is None else (lambda k: f"profile {k}: ")
+        extents = [g._extents if g.smoothing_filter is not None else (0, 0) for g in gates]
+        for k, (g, (nf, nt)) in enumerate(zip(gates, extents)):
+            reason = _rows_smoothing_refusal(nf, nt, True)
+            if reason:
+                raise NotImplementedError(f"{self._api}: {where(k)}freq_mask_smooth_hz={g.freq_mask_smooth_hz} / "
+                                          f"time_mask_smooth_ms={g.time_mask_smooth_ms} give smoothing extents ({nf}, {nt}) "
+                                          f"bins / frames, {reason}")
         if isinstance(n_rows, bool) or not isinstance(n_rows, (int, np.integer)) or n_rows < 1:
             raise ValueError(f"n_rows must be a positive int, got {n_rows!r}")
-        n = int(tg.n_movemean_nonstationary)
-        if n < 1:
-            raise ValueError(f"n_movemean_nonstationary must be at least 1, got {n}")
+        for k, g in enumerate(gates):
+            if int(g.n_movemean_nonstationary) < 1:
+                raise ValueError(f"{where(k)}n_movemean_nonstationary must be at least 1, got {int(g.n_movemean_nonstationary)}")
         self.n_rows = int(n_rows)
-        self._gate_kw = dict(nf=nf, nt=nt, params=tg._params(), window=torch.hann_window(tg.win_length).numpy())
+        nf, nt = extents[0]
+        self._gate_kw = dict(nf=nf, nt=nt, params=gates[0]._params(), window=torch.hann_window(tg.win_length).numpy())
+        # b200gate_tprofile of every profile, derived as _open derives a handle's settings (None: the handle's own)
+        self._profiles = None if profiles is None else [
+            (nf_k, nt_k, int(g.n_movemean_nonstationary), float(g.n_thresh_nonstationary),
+             1.0 / float(g.temp_coeff_nonstationary), float(g.prop_decrease)) for g, (nf_k, nt_k) in zip(gates, extents)]
         self._lib = _lib
         self._hop, self._n_fft, self._win = tg.hop_length, tg.n_fft, tg.win_length
-        self._right, self._nt = n - 1 - (n - 1) // 2, nt
-        e = 1 if (self._right + nt) % 2 == 0 else 0
-        self.latency_samples = self._n_fft // 2 + self._hop * (self._right + nt + 4 + e) - 1
+        n = [int(g.n_movemean_nonstationary) for g in gates]
+        self._right_k = np.array([v - 1 - (v - 1) // 2 for v in n], dtype=np.int64)
+        self._nt_k = np.array([e[1] for e in extents], dtype=np.int64)
+        self._right, self._nt = int(self._right_k[0]), int(self._nt_k[0])
+        self.latency_samples_per_profile = [
+            self._n_fft // 2 + self._hop * (int(r) + int(t) + 4 + (1 if (r + t) % 2 == 0 else 0)) - 1
+            for r, t in zip(self._right_k, self._nt_k)]
+        self.latency_samples = max(self.latency_samples_per_profile)
         self._gate = None
         self._device = self._dtype = None
 
-    def returned_after(self, R: int) -> int:
-        """samples_returned after R samples per row (the closed form above)."""
+    def returned_after(self, R: int, profile: int = 0) -> int:
+        """samples_returned after R samples per row (the closed form above) of a row on profile `profile`."""
+        if isinstance(profile, bool) or not isinstance(profile, (int, np.integer)) or not 0 <= profile < len(self._nt_k):
+            raise ValueError(f"profile must be an int in [0, {len(self._nt_k)}), got {profile!r}")
         if R < self._n_fft // 2:
             return 0
         c = (R - self._n_fft // 2) // self._hop + 1
-        nS = (c - c % 2) - 1 - self._right - self._nt
+        nS = (c - c % 2) - 1 - int(self._right_k[profile]) - int(self._nt_k[profile])
         hb = nS - nS % 2
         return self._hop * max(0, hb - 2)
 
@@ -311,6 +328,8 @@ class _LiveGate:
             sr=float(sr), prop_decrease=prop, top_db=40.0, n_movemean=n_mm, thresh_n_mult=n_thresh,
             sigmoid_slope=1.0 / temp, path_flags=0)
         gate.set_window(self._gate_kw["window"])
+        if self._profiles is not None:
+            gate.tstream_set_profiles(self._profiles)
         gate.tstream_begin(self.n_rows)
         self._gate = gate
 
@@ -435,13 +454,28 @@ class TorchGateSessions(_LiveGate):
     TorchGate.stream(): NotImplementedError for other settings, before any library handle is made.  ValueError, before
     any work: bad lengths (count, negative, larger than n, not integers), rows out of range or repeated, use after
     close().  end() of a row holding fewer than 2 * win_length samples raises the reference's
-    Exception("x must be bigger than 2048") and changes no row."""
+    Exception("x must be bigger than 2048") and changes no row.
+
+    Profiles: sessions(n_rows, profiles=[dict(sr=8000), dict(sr=48000, prop_decrease=0.7), ...]) gates each row with
+    the settings of its profile: the module's, overridden by the profile's keys, which may be sr,
+    prop_decrease, n_thresh_nonstationary, temp_coeff_nonstationary, n_movemean_nonstationary, freq_mask_smooth_hz and
+    time_mask_smooth_ms (the gate type and the STFT geometry stay the module's).  Every row starts on profile 0 and
+    keeps its profile across sessions until assign(rows, profile) moves rows whose current session is empty (new, or
+    after end() / reset()).  A session of a row on profile k equals
+    TorchGate(nonstationary=True, **module settings overridden by profile k)(x_s[None])[0] in every bit, as above;
+    its counts are returned_after(R, profile=k), and latency_samples_per_profile[k] bounds what it holds back
+    (latency_samples is the largest of them).  The device memory is fixed at the first push by n_rows and the
+    profiles.  Refused before any library handle is made: a profile whose settings the module itself would be refused
+    with, with NotImplementedError naming the profile; unknown keys and values TorchGate rejects (prop_decrease
+    outside [0, 1], n_movemean_nonstationary < 1, smoothing below one bin or frame at the profile's sr), with
+    ValueError naming the profile.  Without profiles= there is one profile, the module's own settings."""
     _api, _cls = "TorchGate.sessions()", "TorchGateSessions"
 
-    def __init__(self, tg: "TorchGate", n_rows: int, _lib=None):
-        super().__init__(tg, n_rows, _lib)
+    def __init__(self, tg: "TorchGate", n_rows: int, profiles=None, _lib=None):
+        super().__init__(tg, n_rows, _lib, profiles)
         self._R = np.zeros(self.n_rows, dtype=np.int64)
         self._E = np.zeros(self.n_rows, dtype=np.int64)
+        self._prof = np.zeros(self.n_rows, dtype=np.int64)     # each row's profile
         self._closed = False
 
     @property
@@ -453,9 +487,9 @@ class TorchGateSessions(_LiveGate):
         return self._E.tolist()
 
     def _returned_after_rows(self, R: np.ndarray) -> np.ndarray:
-        """returned_after of every entry of R."""
+        """returned_after of every entry of R, row b on its own profile."""
         c = (R - self._n_fft // 2) // self._hop + 1
-        nS = (c - c % 2) - 1 - self._right - self._nt
+        nS = (c - c % 2) - 1 - self._right_k[self._prof] - self._nt_k[self._prof]
         hb = nS - nS % 2
         return np.where(R < self._n_fft // 2, 0, self._hop * np.maximum(0, hb - 2))
 
@@ -538,6 +572,24 @@ class TorchGateSessions(_LiveGate):
         self._R[r] = 0
         self._E[r] = 0
 
+    def assign(self, rows, profile: int):
+        """Gate the listed rows' next sessions with profile `profile`; their current sessions must be empty."""
+        self._live("assign")
+        r = self._rows(rows)
+        if isinstance(profile, bool) or not isinstance(profile, (int, np.integer)) or not 0 <= profile < len(self._nt_k):
+            raise ValueError(f"profile must be an int in [0, {len(self._nt_k)}), got {profile!r}")
+        busy = [int(b) for b in r if self._R[b] > 0]
+        if busy:
+            raise ValueError(f"rows {busy} hold a session: end() or reset() them before assign()")
+        if self._gate is not None and r.size:
+            self._gate.tstream_assign_rows(r, int(profile))
+        self._prof[r] = profile
+
+    def _open(self, block):
+        super()._open(block)
+        for k in np.unique(self._prof[self._prof != 0]):
+            self._gate.tstream_assign_rows(np.nonzero(self._prof == k)[0].astype(np.int64), int(k))
+
     def close(self):
         """Release the library handle (waits for the device).  Calling it again does nothing."""
         if self._gate is not None:
@@ -571,6 +623,38 @@ def _rows(x, y, lengths):
     """b200gate_row tuples (in, out, n, channels = 1) for float32 rows of x and y with unit sample stride."""
     xs, ys = x.stride(0) * 4, y.stride(0) * 4
     return [(x.data_ptr() + b * xs, y.data_ptr() + b * ys, int(n), 1) for b, n in enumerate(lengths)]
+
+
+_PROFILE_KEYS = ("sr", "prop_decrease", "n_thresh_nonstationary", "temp_coeff_nonstationary", "n_movemean_nonstationary",
+                 "freq_mask_smooth_hz", "time_mask_smooth_ms")
+
+
+def _profile_gates(tg, profiles):
+    """One TorchGate per profile of TorchGate.sessions(profiles=...): tg's settings overridden by the profile's keys.
+    Raises ValueError, naming the profile, for what is not a profile and for values TorchGate rejects."""
+    if isinstance(profiles, (dict, str)) or not hasattr(profiles, "__len__") or len(profiles) == 0:
+        raise ValueError(f"profiles must be a non-empty list of dicts, got {profiles!r}")
+    gates = []
+    for k, p in enumerate(profiles):
+        if not isinstance(p, dict):
+            raise ValueError(f"profile {k}: a profile is a dict of settings, got {p!r}")
+        unknown = sorted(set(p) - set(_PROFILE_KEYS), key=str)
+        if unknown:
+            raise ValueError(f"profile {k}: unknown key(s) {unknown}; a profile may set {', '.join(_PROFILE_KEYS)}")
+        kw = dict(sr=tg.sr, n_std_thresh_stationary=tg.n_std_thresh_stationary, n_thresh_nonstationary=tg.n_thresh_nonstationary,
+                  temp_coeff_nonstationary=tg.temp_coeff_nonstationary, n_movemean_nonstationary=tg.n_movemean_nonstationary,
+                  prop_decrease=tg.prop_decrease, n_fft=tg.n_fft, win_length=tg.win_length, hop_length=tg.hop_length,
+                  freq_mask_smooth_hz=tg.freq_mask_smooth_hz, time_mask_smooth_ms=tg.time_mask_smooth_ms)
+        kw.update(p)
+        if not 0.0 <= kw["prop_decrease"] <= 1.0:
+            raise ValueError(f"profile {k}: prop_decrease must lie in [0, 1], got {kw['prop_decrease']!r}")
+        if kw["temp_coeff_nonstationary"] == 0:
+            raise ValueError(f"profile {k}: temp_coeff_nonstationary must not be 0")
+        try:
+            gates.append(TorchGate(nonstationary=True, **kw))
+        except ValueError as e:
+            raise ValueError(f"profile {k}: {e}") from None
+    return gates
 
 
 def _rows_smoothing_refusal(nf, nt, nonstationary, f_pad=544, smem=200 * 1024):
